@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Headline benchmark: YOLOX-s 640x640 forward+backward images/s on N B200s (BASELINE.json metric), one JSON line.
+"""Headline benchmark: YOLOX-s 640x640 forward+backward images/s on N H100s (BASELINE.json metric), one JSON line.
 
     python bench.py --gpus N --steps K --warmup W            # this repo (libyb200.so kernels)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path (oracle port) on the host cores
+    python bench.py ... --dump-outputs DIR                    # also write what the last timed step computed, DIR/<name>.npy
 
 A "step" = one pass of the hot path over one synthetic COCO-shaped batch per GPU: uint8->Focus preprocessing, CSPDarknet,
 YOLOPAFPN, YOLOX head, SimOTA assignment, IoU/BCE losses and the full backward (data + weight + BN gradients); for N > 1
@@ -30,17 +31,19 @@ FLOP_PER_IMAGE = 79.35e9  # SURVEY.md par.8d: 26.69 fwd + 52.66 bwd GFLOP
 
 
 def peaks():
+    """roofline denominators: MEASURED_PEAKS.json when present, else NVIDIA's H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense bf16 at
+    700 W) -- a ceiling, not a rate this code has been measured to reach"""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as fh:
             d = json.load(fh)
-        return dict(hbm=d.get("hbm_gbs", 6650.0), tf_burst=d.get("bf16_tflops", 1590.0), tf_sust=d.get("bf16_tflops_sustained", 1400.0),
+        return dict(hbm=d.get("hbm_gbs", 3350.0), tf_burst=d.get("bf16_tflops", 989.0), tf_sust=d.get("bf16_tflops_sustained", 989.0),
                     source="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, source="fallback")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region"""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -320,6 +323,29 @@ def yolox_convnext_step(torch, dist, dev, rank, world, batch, steps, warmup, wit
     return out
 
 
+def dump_outputs(out_dir, eng, torch):
+    """What the timed step handed its caller in the last timed step, as DIR/<name>.npy: the six loss values (float64), the decoded head
+    outputs, the flat gradient and the flat parameters after the optimizer step (float32).  Arrays above 4 M entries are replaced by a fixed,
+    seeded sample of 4 M entries (the same positions in every run), so the files stay under 64 MB in all and two builds can be compared."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    cap = 1 << 22
+
+    def sample(t, seed):
+        flat = t.detach().reshape(-1)
+        if flat.numel() <= cap:
+            return flat
+        idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(seed))[:cap].sort().values
+        return flat[idx.to(flat.device)]
+
+    arrays = {"losses": eng.losses.detach().double(), "head_outputs": sample(eng.outputs, 1), "flat_grad": sample(eng.flat_grad, 2),
+              "flat_param": sample(eng.flat_param, 3)}
+    for name, t in arrays.items():
+        a = t.cpu().numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), a if a.dtype == np.float64 else a.astype(np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -337,7 +363,10 @@ def main():
                     help="yolox_s = the headline metric (BASELINE.json configs[1]); yolox_convnext = configs[2] (32 images per GPU; `--gpus 8` = bs 256)")
     ap.add_argument("--no-prefetch", action="store_true", help="e2e leg: copy each batch inside forward() (serial), as the reference does")
     ap.add_argument("--no-optimizer", action="store_true", help="time forward+backward(+all-reduce) only, without the fused SGD step")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step computed to DIR/<name>.npy (yolox_s)")
     args = ap.parse_args()
+    if args.dump_outputs and args.workload != "yolox_s":
+        ap.error("--dump-outputs writes the outputs of the yolox_s step; it is not implemented for --workload %s" % args.workload)
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -471,6 +500,8 @@ def main():
         ms = float(t)
     clocks = sampler.stop() if sampler else None
     value = world * B * args.steps / (ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, torch)
 
     # ---- roofline: every C-ABI call of the step timed live with CUDA events on the launch stream (eager launches, weight gradients serialised
     # on the same stream), grouped into kernel classes; the class with the LARGEST summed time is the one reported ----
@@ -654,7 +685,7 @@ def main():
                 "config": {"workload": WORKLOAD, "global_batch": world * B, "parallelism": f"dp{world}", "cuda_graph": graph is not None,
                            "optimizer": None if opt is None else "fused SGD step inside the timed step (momentum 0.9, wd 5e-4, lr %g)" % BENCH_LR,
                            "allreduce": None if world == 1 else "3 gradient buckets (head / neck / backbone+BN), NCCL all-reduce of each overlapped with the backward of the next range",
-                           "l2": "per-step working set (~%.0f GB of activations and gradients) exceeds the 126 MB L2; no explicit flush" % (0.245 * B)},
+                           "l2": "per-step working set (~%.0f GB of activations and gradients) exceeds the 50 MB L2; no explicit flush" % (0.245 * B)},
                 "clocks": clocks, "e2e": e2e, "gpu_launches": (launches_per_step + (1 if opt is not None else 0)) * args.steps, "roofline": roof, "kernel_classes": classes, "slowest_calls": top_calls if rank == 0 else None, "cpu_baseline": cpu, "library_bar": lib_bar, "nms": nms, "convnext": cnx_line,
                 "loss": final_loss}
         print(json.dumps(line), flush=True)

@@ -1,4 +1,4 @@
-/* yb200 -- C ABI of the B200 (sm_100a) YOLOX hot path.
+/* yb200 -- C ABI of the H100 (sm_90a) YOLOX hot path.
  *
  * The reference (lucasjinreal/yolov7_d2) has no FFI of its own: every entry point below replaces a
  * PyTorch / torchvision call the reference makes on its hot path (file:line cited per function, paths
@@ -45,7 +45,7 @@ const char* yb200_last_error(void);
 int yb200_pack_conv_weight(const float* w_oihw, int cout, int cin, int ksize, int cout_pad, int cin_pad,
                            void* w_fwd, void* w_dgrad, void* stream);
 
-/* ---- convolution (implicit GEMM on tcgen05) ------------------------------------------------------ */
+/* ---- convolution (implicit GEMM on wgmma) -------------------------------------------------------- */
 /* z = conv2d(x, w) without bias, padding (k-1)/2 -- BaseConv.conv, wrappers.py:67-80.
  * ksize in {1,3}, stride in {1,2} (stride 2 only with ksize 3).  z is the pre-BatchNorm output, stored as **fp16**
  * (same 2-byte NHWC view; BatchNorm's mean subtraction makes this tensor the precision-critical one).
@@ -227,7 +227,7 @@ int yb200_pack_conv_weights_batched(const yb200_pack_desc* table_dev, const int6
 /* SPLIT storage: an activation a is the sum of `planes` bf16 values a0 = bf16(a), a1 = bf16(a - a0) [, a2 = bf16(a - a0 - a1)]:
  * 16 significant bits with planes = 2, the full 24 bits of fp32 with planes = 3.  All planes live in one NHWC bf16 buffer,
  * lo_delta channels apart, so a yb200_act describes plane 0 and (view, lo_delta, planes) the value.  The convolution keeps
- * every partial product a_i * w_j with i + j < planes (3 / 6 taps per spatial tap of the SAME tcgen05 implicit GEMM, one
+ * every partial product a_i * w_j with i + j < planes (3 / 6 taps per spatial tap of the SAME wgmma implicit GEMM, one
  * fp32 accumulator); the pre-BatchNorm output z is fp32 NHWC [n][h/stride][w/stride][z_pitch], channels [z_off, z_off+cout).
  * Used to check the reference's fp32 logits / losses to 1e-3 (tests/test_strict_gpu.py); forward only.
  * yb200_pack_conv_weight_split: fp32 OIHW -> [cout_pad][planes][k*k][cin_pad], `nn.Conv2d.weight` of wrappers.py:67-75.
@@ -376,7 +376,7 @@ int yb200_sigmoid(const yb200_act* x, const yb200_act* out, void* stream);
  * yb200_conv2d_wgrad(x = features, dz = iam_prob, ksize 1) (the pixel contraction of :74), normalizer = yb200_colsum(iam_prob).              */
 int yb200_iam_normalize(const float* raw, const float* normalizer, int rows, int cols, const yb200_act* out, void* stream);
 /* Backward of yb200_attention_fwd: given out, its gradient dout and the saved lse, dq / dk / dv (bf16 views shaped like q / k / k; they may be
- * slices of one packed buffer).  P is recomputed from lse; two kernels (per key tile: dK, dV; per query tile: dQ), accumulation in TMEM,
+ * slices of one packed buffer).  P is recomputed from lse; two kernels (per key tile: dK, dV; per query tile: dQ), accumulation in registers,
  * no atomics.  workspace: yb200_attention_bwd_workspace(q) bytes (D = <dout, out> per query row and head).                                     */
 int64_t yb200_attention_bwd_workspace(const yb200_act* q);
 int yb200_attention_bwd(const yb200_act* q, const yb200_act* k, const yb200_act* v, const yb200_act* out, const yb200_act* dout,

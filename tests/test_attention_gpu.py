@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 attention core (yb200_attention_fwd) against the oracle's attention_core (= the arithmetic inside
+"""GPU parity of the wgmma attention core (yb200_attention_fwd) against the oracle's attention_core (= the arithmetic inside
 torch's nn.MultiheadAttention that detr_backbone.py:140,200-202 instantiates) on the same bf16-rounded q, k, v.
 Tolerance: probabilities and the output are rounded to bf16 (rel 2^-8 each) => 2^-6 of the output's max; the log-sum-exp is fp32 => 2e-3 abs."""
 import ctypes

@@ -33,7 +33,7 @@ def test_argument_validation_without_gpu():
     assert L.yb200_simota_workspace(64, 8400) > 0 and L.yb200_nms_workspace(64, 8400) > 0
 
 
-def test_sass_contains_blackwell_tensor_and_tma_instructions():
+def test_sass_contains_hopper_tensor_and_tma_instructions():
     import shutil
     import subprocess
 
@@ -42,12 +42,12 @@ def test_sass_contains_blackwell_tensor_and_tma_instructions():
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not available")
     sass = subprocess.run(["cuobjdump", "-sass", capi.LIB_PATH], capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass and "UTMALDG" in sass and "LDTM" in sass, "tcgen05 / TMA instructions missing from the sm_100a build"
+    assert "HGMMA" in sass and "UTMALDG" in sass, "wgmma / TMA instructions missing from the sm_90a build"
 
 
-def test_attention_and_pair_kernels_use_tensor_memory():
-    """per kernel: the attention core and the CTA-pair convolution must themselves contain tcgen05 MMA / TMA / TMEM-load instructions
-    (not just some other kernel of the library), and the pair kernel the 2-CTA MMA form"""
+def test_attention_and_gemm_kernels_use_wgmma():
+    """per kernel: the attention core, the convolution GEMM and the weight-gradient GEMM must themselves contain warpgroup MMA and TMA
+    instructions (not just some other kernel of the library)"""
     import re
     import shutil
     import subprocess
@@ -61,15 +61,13 @@ def test_attention_and_pair_kernels_use_tensor_memory():
     for part in re.split(r"\n\s*Function : ", sass)[1:]:
         name, _, body = part.partition("\n")
         funcs[name.strip()] = body
-    att = [b for n, b in funcs.items() if "attention_fwd_kernel" in n]
-    assert att, "attention_fwd_kernel not found in the library"
-    assert all("UTCHMMA" in b and "UTMALDG" in b and "LDTM" in b and "MUFU.EX2" in b for b in att)
-    pair = [b for n, b in funcs.items() if "conv_gemm_pair_kernel" in n]
-    assert pair and all("UTCHMMA.2CTA" in b for b in pair), "CTA-pair kernels must issue cta_group::2 MMAs"
+    att = [b for n, b in funcs.items() if "attention_fwd_kernel" in n or "attention_bwd_kv_kernel" in n or "attention_bwd_q_kernel" in n]
+    assert len(att) == 6, "attention kernels not found in the library"
+    assert all("HGMMA" in b and "UTMALDG" in b and "MUFU.EX2" in b for b in att)
+    conv = [b for n, b in funcs.items() if "conv_gemm_persistent_kernel" in n]
+    assert conv and all("HGMMA" in b and "UTMALDG" in b for b in conv)
     wg = [b for n, b in funcs.items() if "wgrad_gemm_kernel" in n]
-    assert wg and all("UTCHMMA" in b for b in wg)
-    staged = [b for n, b in funcs.items() if "conv_gemm_staged_kernel" in n]
-    assert staged and all("UTMASTG" in b for b in staged), "the staged epilogue must store its tile through the TMA unit"
+    assert wg and all("HGMMA" in b and "UTMALDG" in b for b in wg)
     # programmatic dependent launch: every kernel of the library waits for its predecessor (griddepcontrol.wait = ACQBULK) and releases its
     # dependents (launch_dependents = PREEXIT)
     missing = [n for n, b in funcs.items() if "ACQBULK" not in b or "PREEXIT" not in b]

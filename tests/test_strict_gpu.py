@@ -1,8 +1,8 @@
 """north_star: "fp32 losses and logits within 1e-3 relative" -- checked literally, on the GPU, in STRICT mode.
 
-YoloxEngine(strict=True) (or YB200_STRICT=1) runs the same plan on the same tcgen05 implicit-GEMM kernel, but every activation and
+YoloxEngine(strict=True) (or YB200_STRICT=1) runs the same plan on the same wgmma implicit-GEMM kernel, but every activation and
 weight is a sum of three bf16 planes (a0 + a1 + a2 = all 24 significant bits of the fp32 value; csrc/strict.cu; YB200_STRICT_PLANES=2 keeps
-16 bits) multiplied as the six products a_i * w_j with i + j < 3 into the fp32 TMEM accumulator, with fp32 pre-BatchNorm outputs and fp64
+16 bits) multiplied as the six products a_i * w_j with i + j < 3 into the fp32 accumulator, with fp32 pre-BatchNorm outputs and fp64
 batch statistics.  The result is compared with the fp32 CPU oracle
 (oracle/yolox_oracle.py, pinned to the reference by tests/golden/*):
     head outputs (decoded boxes, objectness and class logits): |err| <= 1e-3 * max(1, |ref|)   elementwise

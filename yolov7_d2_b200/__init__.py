@@ -1,2 +1,2 @@
-"""B200-native (sm_100a) YOLOX hot path behind the yolov7_d2 registry surface."""
+"""H100-native (sm_90a) YOLOX hot path behind the yolov7_d2 registry surface."""
 __version__ = "0.1.0"

@@ -1,4 +1,4 @@
-"""ConvNeXt backbone on the B200 kernels: execution plan (ConvNeXtEngine) and the reference-facing module.
+"""ConvNeXt backbone on the H100 kernels: execution plan (ConvNeXtEngine) and the reference-facing module.
 
 Reference: yolov7/modeling/backbone/convnext.py -- `Block` :25-60, `ConvNeXt` :62-180 (forward_features :149-159), `LayerNorm` :182-206,
 `build_convnext_backbone` :209-230.  Parameter names / shapes are the reference's state_dict; parameters and gradients live in flat
@@ -7,7 +7,7 @@ fp32 buffers (same contract as engine.YoloxEngine, so optim.FlatOptimizer and th
 Data layout: NHWC bf16 activations.  Per block the plan keeps x (input), d (depthwise output), per-pixel LayerNorm statistics, y (normalised),
 u (pwconv1 pre-activation), h = GELU(u) and the block output; the 4C-wide du gradient and the C-wide temporaries are shared per stage.
 Kernel sequence of one block (forward 4 launches, backward 11):
-  dwconv7 -> layernorm_fwd -> linear_gelu_fwd (tcgen05 GEMM, bias+GELU epilogue) -> conv2d_affine_fwd (GEMM, gamma*b2 shift + residual epilogue)
+  dwconv7 -> layernorm_fwd -> linear_gelu_fwd (wgmma GEMM, bias+GELU epilogue) -> conv2d_affine_fwd (GEMM, gamma*b2 shift + residual epilogue)
   colsum(dOut) | linear_dgrad_gelu (GEMM, GELU' epilogue, db1 column sums) | wgrad(h, dOut) + layer_scale_grad | dgrad(du) | wgrad(y, du)
   | layernorm_bwd | dwconv7(flip, + dOut) | dwconv7_wgrad
 There is no CPU implementation: every method needs the CUDA library.

@@ -1,19 +1,17 @@
-// Multi-head attention core on tcgen05 (SURVEY.md par.8a row T1): the part of nn.MultiheadAttention between in_proj and out_proj
+// Multi-head attention core on wgmma (SURVEY.md par.8a row T1): the part of nn.MultiheadAttention between in_proj and out_proj
 //   out[b, i, h] = softmax_j( scale * <q[b,i,h], k[b,j,h]> + key_padding_mask[b,j] ) . v[b,j,h]
 // as used by TransformerEncoderLayer / TransformerDecoderLayer (yolov7/modeling/backbone/detr_backbone.py:140,157-161,200-236: d_model 256,
 // 8 heads x 32, sequences of 1050 tokens at 800x1333).  Head dimension 32 is compiled in.
 //
 // One CTA per (128-query tile, head, image); flash-attention style streaming over 128-key tiles:
-//   warp 0     TMA producer: Q tile once, K / V tiles double-buffered (5-D NHWC maps, out-of-range tokens zero-filled)
-//   warp 1     one thread issues S = Q K^T (UMMA 128x128x32, K-major operands) and O_j = P V (UMMA 128x32x128, P from shared memory,
-//              V as MN-major B operand straight from its token-major tile) into TMEM
-//   warps 2-5  online softmax, one query row per thread: tcgen05.ld of S, running max / sum in the exp2 domain, P written as bf16 into a
-//              128B-swizzled K-major tile, running output kept in registers (acc = acc * alpha + O_j)
-// With 32-wide heads the kernel is bound by MUFU.EX2 (128 x 128 exponentials per tile against 2 MFLOP of MMA), so the design goal is
-// simply to keep the exponentials flowing: TMEM holds S (128 columns) and O_j (32 columns); 256 columns are allocated so that two CTAs
-// share an SM and overlap each other's MMA / softmax phases.
+//   warp 4     TMA producer: Q tile once, K / V tiles double-buffered (5-D NHWC maps, out-of-range tokens zero-filled)
+//   warps 0-3  one warpgroup: S = Q K^T (wgmma 64x128x16, K-major operands, 64 query rows at a time) staged as fp32 rows in shared memory,
+//              online softmax with one query row per thread (running max / sum in the exp2 domain), P written as bf16 into a 128B-swizzled
+//              K-major tile, O_j = P V (wgmma 64x32x16, V as MN-major B operand straight from its token-major tile) staged the same way and
+//              folded into the running output kept in registers (acc = (acc + O_j) * alpha)
+// With 32-wide heads the kernel is bound by MUFU.EX2 (128 x 128 exponentials per tile against 2 MFLOP of MMA).
 #include "host_common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 using namespace yb;
 
@@ -21,11 +19,14 @@ namespace {
 
 constexpr int kAttD = 32;          // head dimension
 constexpr int kAttTile = 128;      // queries per CTA, keys per step
-constexpr int kAttThreads = 192;
+constexpr int kAttThreads = 160;   // one compute warpgroup + one producer warp
 constexpr int kQBytes = kAttTile * kAttD * 2;       // 8 KB, 64-byte rows (swizzle 64)
 constexpr int kKVBytes = kAttTile * kAttD * 2;
 constexpr int kPBytes = kAttTile * kAttTile * 2;    // 32 KB: two K-blocks of [128 rows][64 keys] with 128-byte rows (swizzle 128)
-constexpr int kAttSmem = kQBytes + 4 * kKVBytes + kPBytes + 1024;
+constexpr int kSPitch = kAttTile + 4;               // fp32 row pitch of a staged score tile (16-byte aligned, conflict-free row reads)
+constexpr int kOPitch = kAttD + 4;                  // fp32 row pitch of a staged [128][32] output tile
+constexpr int kSBytes = kAttTile * kSPitch * 4;     // 66 KB: staged S (forward), later the staged O_j
+constexpr int kAttSmem = kQBytes + 4 * kKVBytes + kPBytes + kSBytes + 1024;
 
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ float ex2(float x) {
@@ -64,21 +65,20 @@ struct AttnParams {
 
 template <bool DROP>  // the dropout-free instantiation is the kernel as it was (the extra integer work and registers cost the p = 0 path 35 % when the
                       // choice was a run-time branch inside the softmax loop)
-__global__ void __launch_bounds__(kAttThreads)
+__global__ void __launch_bounds__(kAttThreads, 1)
 attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                      const __grid_constant__ AttnParams p) {
   pdl_sync();
   extern __shared__ uint8_t smem_dyn[];
-  __shared__ __align__(8) uint64_t s_bar[8];  // q_full, kv_full[2], kv_empty[2], s_full, p_ready, o_full
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t s_bar[5];  // q_full, kv_full[2], kv_empty[2]
   __shared__ __align__(16) float s_bias[2][kAttTile];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = warp_id_uniform();
   const int q0 = blockIdx.x * kAttTile, h = blockIdx.y, b = blockIdx.z;
   const uint32_t base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
   const uint32_t sQ = base, sK = base + kQBytes, sV = sK + 2 * kKVBytes, sP = sV + 2 * kKVBytes;
+  float* const sS = reinterpret_cast<float*>(smem_dyn + (sP + kPBytes - smem_u32(smem_dyn)));
   const uint32_t bar_q = smem_u32(&s_bar[0]), bar_kv_full = smem_u32(&s_bar[1]), bar_kv_empty = smem_u32(&s_bar[3]);
-  const uint32_t bar_s = smem_u32(&s_bar[5]), bar_p = smem_u32(&s_bar[6]), bar_o = smem_u32(&s_bar[7]);
   const int ntiles = (p.lk + kAttTile - 1) / kAttTile;
 
   if (threadIdx.x == 0) {
@@ -87,18 +87,11 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       mbar_init(bar_kv_full + 8 * s, 1);
       mbar_init(bar_kv_empty + 8 * s, 1);
     }
-    mbar_init(bar_s, 1);
-    mbar_init(bar_p, kAttTile);  // every softmax thread arrives
-    mbar_init(bar_o, 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc<256>(smem_u32(&s_tmem));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_s = s_tmem, tmem_o = s_tmem + 128;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (elect_one()) {
       tma_prefetch_desc(&tmQ);
       tma_prefetch_desc(&tmK);
@@ -113,79 +106,63 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         tma_load_5d(sV + st * kKVBytes, &tmV, bar_kv_full + 8 * st, p.v_coff + h * kAttD, j * kAttTile, 0, 0, b);
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      const uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);
-      const uint32_t idesc_o = umma_idesc_bf16(128, kAttD, 0, 1);  // B = V tile, MN-major (head dimension contiguous)
-      const uint32_t l64 = umma_layout_code(64), l128 = umma_layout_code(128);
-      mbar_wait(bar_q, 0);
-      for (int j = 0; j < ntiles; ++j) {
-        const int st = j & 1;
-        mbar_wait(bar_kv_full + 8 * st, (j >> 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < kAttD / 16; ++k)
-          umma_f16(tmem_s, umma_smem_desc(sQ + k * 32, 16, 512, l64), umma_smem_desc(sK + st * kKVBytes + k * 32, 16, 512, l64), idesc_s, k != 0 ? 1u : 0u);
-        umma_commit(bar_s);
-        mbar_wait(bar_p, j & 1);  // P_j is in shared memory (and the softmax threads are done with S_j and O_{j-1})
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < kAttTile / 16; ++kk) {
-          const uint64_t da = umma_smem_desc(sP + (kk >> 2) * (kAttTile * 128) + (kk & 3) * 32, 16, 1024, l128);
-          const uint64_t db = umma_smem_desc(sV + st * kKVBytes + kk * 16 * (kAttD * 2), kKVBytes, 8 * (kAttD * 2), l64);
-          umma_f16(tmem_o, da, db, idesc_o, kk != 0 ? 1u : 0u);
-        }
-        umma_commit(bar_o);
-        umma_commit(bar_kv_empty + 8 * st);
-      }
-    }
-  } else {
-    const int quad = warp & 3;            // TMEM lane quadrant this warp may read
-    const int row = quad * 32 + lane;     // query row of this thread inside the tile
-    const int tid = threadIdx.x - 64;     // 0..127 among the softmax threads
-    const uint32_t lane_base = static_cast<uint32_t>(quad * 32) << 16;
+  } else if (warp < 4) {
+    const int row = threadIdx.x;  // query row of this thread inside the tile
+    const int tid = threadIdx.x;
+    const uint32_t l64 = gmma_layout_code(64), l128 = gmma_layout_code(128);
+    const float* const srow = sS + row * kSPitch;
     float m = -INFINITY, l = 0.f;
     uint32_t drop_key = 0;
     if constexpr (DROP) drop_key = drop_row_key(p.drop.seed, static_cast<uint32_t>(b * p.heads + h), static_cast<uint32_t>(q0 + row));
     float acc[kAttD];
 #pragma unroll
     for (int i = 0; i < kAttD; ++i) acc[i] = 0.f;
+    mbar_wait(bar_q, 0);
     for (int j = 0; j < ntiles; ++j) {
+      const int st = j & 1;
       {  // additive mask of this key tile: 0 or -inf (padding keys and keys beyond lk)
         const int key = j * kAttTile + tid;
         const bool dead = key >= p.lk || (p.mask != nullptr && p.mask[static_cast<size_t>(b) * p.lk + key] != 0);
         s_bias[j & 1][tid] = dead ? -INFINITY : 0.f;
       }
-      named_bar_sync(1, kAttTile);
+      named_bar_sync(1, kAttTile);  // also: every thread is done with the previous tile's staged O_j
       const float* bias = s_bias[j & 1];
-      mbar_wait(bar_s, j & 1);
-      tc_fence_after();
+      mbar_wait(bar_kv_full + 8 * st, (j >> 1) & 1);
+      // S = Q K^T, 64 query rows per wgmma, staged as fp32 rows
+#pragma unroll 1
+      for (int hf = 0; hf < 2; ++hf) {
+        float sacc[kAttTile / 2];
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kAttD / 16; ++k)
+          Wgmma<kAttTile>::mma<0, 0>(sacc, gmma_desc(sQ + hf * 64 * (kAttD * 2) + k * 32, 16, 512, l64),
+                                     gmma_desc(sK + st * kKVBytes + k * 32, 16, 512, l64), k != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operand(sacc);
+        wg_acc_to_smem<kAttTile>(sacc, sS + hf * 64 * kSPitch, kSPitch);
+      }
+      named_bar_sync(1, kAttTile);
       // pass 1: row maximum of the scaled, masked scores
       float mx = m;
 #pragma unroll 1
       for (int c = 0; c < kAttTile; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_s + lane_base + c, r);
-        tmem_ld_wait();
+        float r[32];
+        lds_row32(srow + c, r);
 #pragma unroll
         for (int i = 0; i < 32; i += 4) {  // 16-byte broadcast loads of the mask bias: per-element LDS made the LSU the busiest pipe
           const float4 bb = *reinterpret_cast<const float4*>(bias + c + i);
-          mx = fmaxf(mx, fmaf(__uint_as_float(r[i]), p.scale_log2, bb.x));
-          mx = fmaxf(mx, fmaf(__uint_as_float(r[i + 1]), p.scale_log2, bb.y));
-          mx = fmaxf(mx, fmaf(__uint_as_float(r[i + 2]), p.scale_log2, bb.z));
-          mx = fmaxf(mx, fmaf(__uint_as_float(r[i + 3]), p.scale_log2, bb.w));
+          mx = fmaxf(mx, fmaf(r[i], p.scale_log2, bb.x));
+          mx = fmaxf(mx, fmaf(r[i + 1], p.scale_log2, bb.y));
+          mx = fmaxf(mx, fmaf(r[i + 2], p.scale_log2, bb.z));
+          mx = fmaxf(mx, fmaf(r[i + 3], p.scale_log2, bb.w));
         }
       }
       const float m_safe = mx == -INFINITY ? 0.f : mx;  // every key so far is masked: keep everything at zero without NaNs
       const float alpha = ex2(m - m_safe);               // m = -inf -> 0
-      if (j > 0) {  // fold the previous tile's P V product in before P / O are overwritten
-        mbar_wait(bar_o, (j - 1) & 1);
-        tc_fence_after();
-        uint32_t o[32];
-        tmem_ld_32x32(tmem_o + lane_base, o);
-        tmem_ld_wait();
+      if (j > 0) {  // the previous tile's P V product is already folded into acc
 #pragma unroll
-        for (int i = 0; i < kAttD; ++i) acc[i] = (acc[i] + __uint_as_float(o[i])) * alpha;
+        for (int i = 0; i < kAttD; ++i) acc[i] *= alpha;
       }
       l *= alpha;
       m = mx;
@@ -193,17 +170,16 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       float rowsum = 0.f;
 #pragma unroll 1
       for (int c = 0; c < kAttTile; c += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_s + lane_base + c, r);
-        tmem_ld_wait();
+        float r[32];
+        lds_row32(srow + c, r);
         uint32_t pk[16];
 #pragma unroll
         for (int i = 0; i < 32; i += 4) {
           const float4 bb = *reinterpret_cast<const float4*>(bias + c + i);
-          const float p0 = ex2(fmaf(__uint_as_float(r[i]), p.scale_log2, bb.x - m_safe));
-          const float p1 = ex2(fmaf(__uint_as_float(r[i + 1]), p.scale_log2, bb.y - m_safe));
-          const float p2 = ex2(fmaf(__uint_as_float(r[i + 2]), p.scale_log2, bb.z - m_safe));
-          const float p3 = ex2(fmaf(__uint_as_float(r[i + 3]), p.scale_log2, bb.w - m_safe));
+          const float p0 = ex2(fmaf(r[i], p.scale_log2, bb.x - m_safe));
+          const float p1 = ex2(fmaf(r[i + 1], p.scale_log2, bb.y - m_safe));
+          const float p2 = ex2(fmaf(r[i + 2], p.scale_log2, bb.z - m_safe));
+          const float p3 = ex2(fmaf(r[i + 3], p.scale_log2, bb.w - m_safe));
           rowsum += (p0 + p1) + (p2 + p3);  // the normaliser is the sum of the UNDROPPED probabilities: dropout(softmax(S)) V
           if constexpr (DROP) {
             const uint32_t col = static_cast<uint32_t>(j * kAttTile + c + i);
@@ -224,19 +200,31 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         }
       }
       l += rowsum;
-      fence_proxy_async();   // generic-proxy writes of P must be visible to the tensor core (async proxy)
-      tc_fence_before();     // and this thread's TMEM reads are ordered before the MMA that overwrites S / O
-      mbar_arrive(bar_p);
-    }
-    // last P V product
-    mbar_wait(bar_o, (ntiles - 1) & 1);
-    tc_fence_after();
-    {
-      uint32_t o[32];
-      tmem_ld_32x32(tmem_o + lane_base, o);
-      tmem_ld_wait();
+      fence_proxy_async();  // generic-proxy writes of P must be visible to the tensor core (async proxy)
+      named_bar_sync(1, kAttTile);
+      // O_j = P V (64 query rows per wgmma), staged over the scores (no longer read) and folded into acc
+      float o[2][kAttD / 2];
+      wgmma_fence();
 #pragma unroll
-      for (int i = 0; i < kAttD; ++i) acc[i] += __uint_as_float(o[i]);
+      for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+        for (int kk = 0; kk < kAttTile / 16; ++kk)
+          Wgmma<kAttD>::mma<0, 1>(o[hf], gmma_desc(sP + (kk >> 2) * (kAttTile * 128) + hf * 64 * 128 + (kk & 3) * 32, 16, 1024, l128),
+                                  gmma_desc(sV + st * kKVBytes + kk * 16 * (kAttD * 2), kKVBytes, 8 * (kAttD * 2), l64), kk != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operand(o[0]);
+      wgmma_fence_operand(o[1]);
+      if (threadIdx.x == 0) mbar_arrive(bar_kv_empty + 8 * st);
+      wg_acc_to_smem<kAttD>(o[0], sS, kOPitch);
+      wg_acc_to_smem<kAttD>(o[1], sS + 64 * kOPitch, kOPitch);
+      named_bar_sync(1, kAttTile);
+      {
+        float ov[kAttD];
+        lds_row32(sS + row * kOPitch, ov);
+#pragma unroll
+        for (int i = 0; i < kAttD; ++i) acc[i] += ov[i];
+      }
     }
     const int qi = q0 + row;
     if (qi < p.lq) {
@@ -254,20 +242,16 @@ attention_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       if (p.lse != nullptr) p.lse[(static_cast<size_t>(b) * p.heads + h) * p.lq + qi] = l > 0.f ? (m + log2f(l)) * 0.6931471805599453f : -INFINITY;
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<256>(s_tmem);
 }
 
 // ================================================================================================================================
 // Backward of the attention core.  With P = softmax(S), S = scale * Q K^T + mask, O = P V and D_i = <dO_i, O_i>:
 //   dV = P^T dO,   dP = dO V^T,   dS = P o (dP - D) * scale,   dQ = dS K,   dK = dS^T Q
 // P is recomputed from the saved log-sum-exp (fp32 per query row).  Two kernels, no atomics (bit-reproducible):
-//   attention_bwd_kv_kernel  one CTA per (128-key tile, head, image), streams over query tiles, dK / dV accumulate in TMEM
-//   attention_bwd_q_kernel   one CTA per (128-query tile, head, image), streams over key tiles, dQ accumulates in TMEM
-// Operand forms (all already used by the forward kernel or the weight-gradient GEMM): S and dP are K-major x K-major UMMAs on the TMA tiles;
-// P / dS are written by the softmax threads as bf16 [query][key] tiles (128-byte rows, swizzle 128) and consumed either K-major (dQ = dS K)
+//   attention_bwd_kv_kernel  one CTA per (128-key tile, head, image), streams over query tiles, dK / dV accumulate in registers
+//   attention_bwd_q_kernel   one CTA per (128-query tile, head, image), streams over key tiles, dQ accumulates in registers
+// Operand forms: S and dP are K-major x K-major wgmmas on the TMA tiles, 64 query rows at a time, staged as fp32 rows in shared memory;
+// P / dS are written by the compute threads as bf16 [query][key] tiles (128-byte rows, swizzle 128) and consumed either K-major (dQ = dS K)
 // or MN-major (dV = P^T dO, dK = dS^T Q: the contraction index is the tile row); dO / Q / K enter those products as MN-major B operands
 // straight from their token-major tiles.
 // ================================================================================================================================
@@ -283,8 +267,9 @@ struct AttnBwdParams {
   int dq_pitch, dq_coff, dk_pitch, dk_coff, dv_pitch, dv_coff;
 };
 
-constexpr int kBwdSmemKV = 2 * kKVBytes + 4 * kQBytes + 2 * kPBytes + 1024;  // K, V | Q x2, dO x2 | P, dS
-constexpr int kBwdSmemQ = 2 * kQBytes + 4 * kKVBytes + kPBytes + 1024;       // Q, dO | K x2, V x2 | dS
+constexpr int kBwdStage = 64 * kSPitch * 4;  // one staged [64 query rows][128 keys] fp32 tile (S or dP)
+constexpr int kBwdSmemKV = 2 * kKVBytes + 4 * kQBytes + 2 * kPBytes + 2 * kBwdStage + 1024;  // K, V | Q x2, dO x2 | P, dS | staged S, dP
+constexpr int kBwdSmemQ = 2 * kQBytes + 4 * kKVBytes + kPBytes + 2 * kBwdStage + 1024;       // Q, dO | K x2, V x2 | dS | staged S, dP
 
 // D[b][h][q] = sum_d dO[b][q][h][d] * O[b][q][h][d]
 __global__ void attention_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, int o_pitch, int o_coff, const __nv_bfloat16* __restrict__ d_o, int do_pitch,
@@ -307,25 +292,24 @@ __global__ void attention_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, i
   dsum[(static_cast<size_t>(b) * heads + h) * lq + q] = acc;
 }
 
-// one 32-column chunk of P and dS for the thread's query row: reads S and dP from TMEM, writes both bf16 tiles ([query][key], swizzle 128)
+// one 32-column chunk of P and dS for one query row: reads S and dP from their staged rows, writes both bf16 tiles ([query][key], swizzle 128)
 // With dropout D (0 or 1/(1-p) per element): O = (D o P) V, so the tile written for dV = (D o P)^T dO is the dropped one, dP = D o (dO V^T) and
 // dS = P o (dP - <dO, O>) -- the row term <dO, O> (attention_bwd_prep_kernel) already contains D through O.
 template <bool DROP>
-__device__ __forceinline__ void bwd_chunk(uint32_t tmem_s, uint32_t tmem_dp, uint32_t lane_base, int c, int row, const float* bias, float lse_log2, float dsum,
+__device__ __forceinline__ void bwd_chunk(const float* srow, const float* dprow, int c, int row, const float* bias, float lse_log2, float dsum,
                                           float scale, float scale_log2, uint32_t sP, uint32_t sDS, bool write_p, const DropParams& drop, uint32_t drop_key,
                                           int key0) {
-  uint32_t r[32], g[32];
-  tmem_ld_32x32(tmem_s + lane_base + c, r);
-  tmem_ld_32x32(tmem_dp + lane_base + c, g);
-  tmem_ld_wait();
+  float r[32], g[32];
+  lds_row32(srow + c, r);
+  lds_row32(dprow + c, g);
   uint32_t pk[16], dk[16];
 #pragma unroll
   for (int i = 0; i < 32; i += 4) {
     const float4 bb = *reinterpret_cast<const float4*>(bias + c + i);
-    const float p0 = ex2(fmaf(__uint_as_float(r[i]), scale_log2, bb.x - lse_log2));
-    const float p1 = ex2(fmaf(__uint_as_float(r[i + 1]), scale_log2, bb.y - lse_log2));
-    const float p2 = ex2(fmaf(__uint_as_float(r[i + 2]), scale_log2, bb.z - lse_log2));
-    const float p3 = ex2(fmaf(__uint_as_float(r[i + 3]), scale_log2, bb.w - lse_log2));
+    const float p0 = ex2(fmaf(r[i], scale_log2, bb.x - lse_log2));
+    const float p1 = ex2(fmaf(r[i + 1], scale_log2, bb.y - lse_log2));
+    const float p2 = ex2(fmaf(r[i + 2], scale_log2, bb.z - lse_log2));
+    const float p3 = ex2(fmaf(r[i + 3], scale_log2, bb.w - lse_log2));
     float f0 = 1.f, f1 = 1.f, f2 = 1.f, f3 = 1.f;
     if constexpr (DROP) {
       const uint32_t col = static_cast<uint32_t>(key0 + c + i);
@@ -334,8 +318,8 @@ __device__ __forceinline__ void bwd_chunk(uint32_t tmem_s, uint32_t tmem_dp, uin
     }
     pk[i >> 1] = pack_bf16x2(p0 * f0, p1 * f1);
     pk[(i >> 1) + 1] = pack_bf16x2(p2 * f2, p3 * f3);
-    dk[i >> 1] = pack_bf16x2(p0 * (__uint_as_float(g[i]) * f0 - dsum) * scale, p1 * (__uint_as_float(g[i + 1]) * f1 - dsum) * scale);
-    dk[(i >> 1) + 1] = pack_bf16x2(p2 * (__uint_as_float(g[i + 2]) * f2 - dsum) * scale, p3 * (__uint_as_float(g[i + 3]) * f3 - dsum) * scale);
+    dk[i >> 1] = pack_bf16x2(p0 * (g[i] * f0 - dsum) * scale, p1 * (g[i + 1] * f1 - dsum) * scale);
+    dk[(i >> 1) + 1] = pack_bf16x2(p2 * (g[i + 2] * f2 - dsum) * scale, p3 * (g[i + 3] * f3 - dsum) * scale);
   }
   const uint32_t off = (c >> 6) * (kAttTile * 128) + row * 128;
 #pragma unroll
@@ -348,34 +332,65 @@ __device__ __forceinline__ void bwd_chunk(uint32_t tmem_s, uint32_t tmem_dp, uin
   }
 }
 
-__device__ __forceinline__ void store_row32(__nv_bfloat16* dst, const uint32_t (&o)[32]) {
+__device__ __forceinline__ void store_row32(__nv_bfloat16* dst, const float (&o)[32]) {
 #pragma unroll
   for (int i = 0; i < kAttD; i += 8) {
     uint4 u;
-    u.x = pack_bf16x2(__uint_as_float(o[i]), __uint_as_float(o[i + 1]));
-    u.y = pack_bf16x2(__uint_as_float(o[i + 2]), __uint_as_float(o[i + 3]));
-    u.z = pack_bf16x2(__uint_as_float(o[i + 4]), __uint_as_float(o[i + 5]));
-    u.w = pack_bf16x2(__uint_as_float(o[i + 6]), __uint_as_float(o[i + 7]));
+    u.x = pack_bf16x2(o[i], o[i + 1]);
+    u.y = pack_bf16x2(o[i + 2], o[i + 3]);
+    u.z = pack_bf16x2(o[i + 4], o[i + 5]);
+    u.w = pack_bf16x2(o[i + 6], o[i + 7]);
     *reinterpret_cast<uint4*>(dst + i) = u;
   }
 }
 
+// S and dP of query rows [64 hf, 64 hf + 64) of the tiles at sQ / sDO against the key tiles at sK / sV, staged as fp32 rows
+__device__ __forceinline__ void bwd_scores_half(uint32_t sQ, uint32_t sDO, uint32_t sK, uint32_t sV, int hf, float* stS, float* stDP) {
+  const uint32_t l64 = gmma_layout_code(64);
+  float acc[kAttTile / 2];
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < kAttD / 16; ++k)
+    Wgmma<kAttTile>::mma<0, 0>(acc, gmma_desc(sQ + hf * 64 * (kAttD * 2) + k * 32, 16, 512, l64), gmma_desc(sK + k * 32, 16, 512, l64), k != 0 ? 1u : 0u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_operand(acc);
+  wg_acc_to_smem<kAttTile>(acc, stS, kSPitch);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < kAttD / 16; ++k)
+    Wgmma<kAttTile>::mma<0, 0>(acc, gmma_desc(sDO + hf * 64 * (kAttD * 2) + k * 32, 16, 512, l64), gmma_desc(sV + k * 32, 16, 512, l64), k != 0 ? 1u : 0u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_operand(acc);
+  wg_acc_to_smem<kAttTile>(acc, stDP, kSPitch);
+}
+
+// a [128][32] accumulator held as two 64-row warpgroup fragments -> row `row` of it in `o` (through the staging area at st)
+__device__ __forceinline__ void acc_row32(const float (&a)[2][kAttD / 2], float* st, int row, float (&o)[32]) {
+  named_bar_sync(1, kAttTile);  // the staging area is free
+  wg_acc_to_smem<kAttD>(a[0], st, kOPitch);
+  wg_acc_to_smem<kAttD>(a[1], st + 64 * kOPitch, kOPitch);
+  named_bar_sync(1, kAttTile);
+  lds_row32(st + row * kOPitch, o);
+}
+
 template <bool DROP>
-__global__ void __launch_bounds__(kAttThreads)
+__global__ void __launch_bounds__(kAttThreads, 1)
 attention_bwd_kv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                         const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ AttnBwdParams p) {
   pdl_sync();
   extern __shared__ uint8_t smem_dyn[];
-  __shared__ __align__(8) uint64_t s_bar[8];  // kv_full, qdo_full[2], qdo_empty[2], sdp_full, pds_ready, mma_done
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t s_bar[5];  // kv_full, qdo_full[2], qdo_empty[2]
   __shared__ __align__(16) float s_bias[kAttTile];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = warp_id_uniform();
   const int k0 = blockIdx.x * kAttTile, h = blockIdx.y, b = blockIdx.z;
   const uint32_t base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
   const uint32_t sK = base, sV = sK + kKVBytes, sQ = sV + kKVBytes, sDO = sQ + 2 * kQBytes, sP = sDO + 2 * kQBytes, sDS = sP + kPBytes;
+  float* const stS = reinterpret_cast<float*>(smem_dyn + (sDS + kPBytes - smem_u32(smem_dyn)));
+  float* const stDP = stS + 64 * kSPitch;
   const uint32_t bar_kv = smem_u32(&s_bar[0]), bar_full = smem_u32(&s_bar[1]), bar_empty = smem_u32(&s_bar[3]);
-  const uint32_t bar_sdp = smem_u32(&s_bar[5]), bar_pds = smem_u32(&s_bar[6]), bar_done = smem_u32(&s_bar[7]);
   const int ntiles = (p.lq + kAttTile - 1) / kAttTile;
 
   if (threadIdx.x == 0) {
@@ -384,23 +399,16 @@ attention_bwd_kv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
       mbar_init(bar_full + 8 * s, 1);
       mbar_init(bar_empty + 8 * s, 1);
     }
-    mbar_init(bar_sdp, 1);
-    mbar_init(bar_pds, kAttTile);
-    mbar_init(bar_done, 1);
     mbar_fence_init();
   }
-  if (threadIdx.x >= 64) {  // additive mask of this CTA's key tile
-    const int tid = threadIdx.x - 64, key = k0 + tid;
+  if (threadIdx.x < kAttTile) {  // additive mask of this CTA's key tile
+    const int key = k0 + threadIdx.x;
     const bool dead = key >= p.lk || (p.mask != nullptr && p.mask[static_cast<size_t>(b) * p.lk + key] != 0);
-    s_bias[tid] = dead ? -INFINITY : 0.f;
+    s_bias[threadIdx.x] = dead ? -INFINITY : 0.f;
   }
-  if (warp == 1) tmem_alloc<512>(smem_u32(&s_tmem));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_s = s_tmem, tmem_dp = s_tmem + 128, tmem_dv = s_tmem + 256, tmem_dk = s_tmem + 288;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (elect_one()) {
       mbar_expect_tx(bar_kv, 2 * kKVBytes);
       tma_load_5d(sK, &tmK, bar_kv, p.k_coff + h * kAttD, k0, 0, 0, b);
@@ -413,90 +421,80 @@ attention_bwd_kv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
         tma_load_5d(sDO + st * kQBytes, &tmDO, bar_full + 8 * st, p.do_coff + h * kAttD, i * kAttTile, 0, 0, b);
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      const uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);
-      const uint32_t idesc_t = umma_idesc_bf16(128, kAttD, 1, 1);  // A = P^T / dS^T (MN-major), B = dO / Q tile (MN-major)
-      const uint32_t l64 = umma_layout_code(64), l128 = umma_layout_code(128);
-      mbar_wait(bar_kv, 0);
-      for (int i = 0; i < ntiles; ++i) {
-        const int st = i & 1;
-        mbar_wait(bar_full + 8 * st, (i >> 1) & 1);
-        tc_fence_after();
+  } else if (warp < 4) {
+    const int t = threadIdx.x;
+    const int rl = t & 63, cbeg = (t >> 6) * 64;  // staged row of this thread and the 64 columns of it that it converts
+    const uint32_t l64 = gmma_layout_code(64), l128 = gmma_layout_code(128);
+    float dv[2][kAttD / 2], dk[2][kAttD / 2];  // [key half]: keys [64 g, 64 g + 64) of the tile
 #pragma unroll
-        for (int k = 0; k < kAttD / 16; ++k) {
-          umma_f16(tmem_s, umma_smem_desc(sQ + st * kQBytes + k * 32, 16, 512, l64), umma_smem_desc(sK + k * 32, 16, 512, l64), idesc_s, k != 0 ? 1u : 0u);
-          umma_f16(tmem_dp, umma_smem_desc(sDO + st * kQBytes + k * 32, 16, 512, l64), umma_smem_desc(sV + k * 32, 16, 512, l64), idesc_s, k != 0 ? 1u : 0u);
-        }
-        umma_commit(bar_sdp);
-        mbar_wait(bar_pds, i & 1);
-        tc_fence_after();
+    for (int g = 0; g < 2; ++g)
+#pragma unroll
+      for (int i = 0; i < kAttD / 2; ++i) { dv[g][i] = 0.f; dk[g][i] = 0.f; }
+    mbar_wait(bar_kv, 0);
+    for (int i = 0; i < ntiles; ++i) {
+      const int st = i & 1;
+      mbar_wait(bar_full + 8 * st, (i >> 1) & 1);
+#pragma unroll 1
+      for (int hf = 0; hf < 2; ++hf) {
+        const int row = 64 * hf + rl;
+        const int qi = i * kAttTile + row;
+        const size_t stat = (static_cast<size_t>(b) * p.heads + h) * p.lq + qi;
+        float lse_log2 = qi < p.lq ? p.lse[stat] * 1.4426950408889634f : INFINITY;  // rows beyond lq: p = 0
+        if (lse_log2 == -INFINITY) lse_log2 = INFINITY;                                 // fully masked query: zero gradients instead of NaN
+        const float dsum = qi < p.lq ? p.dsum[stat] : 0.f;
+        uint32_t drop_key = 0;
+        if constexpr (DROP) drop_key = drop_row_key(p.drop.seed, static_cast<uint32_t>(b * p.heads + h), static_cast<uint32_t>(qi));
+        bwd_scores_half(sQ + st * kQBytes, sDO + st * kQBytes, sK, sV, hf, stS, stDP);
+        named_bar_sync(1, kAttTile);
+#pragma unroll 1
+        for (int c = cbeg; c < cbeg + 64; c += 32)
+          bwd_chunk<DROP>(stS + rl * kSPitch, stDP + rl * kSPitch, c, row, s_bias, lse_log2, dsum, p.scale, p.scale_log2, sP, sDS, true, p.drop, drop_key, k0);
+        fence_proxy_async();          // P / dS writes -> visible to the tensor core
+        named_bar_sync(1, kAttTile);  // and the staged tiles are free again
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int g = 0; g < 2; ++g)
 #pragma unroll
         for (int kk = 0; kk < kAttTile / 16; ++kk) {  // contraction over the 128 query rows of the tile, 16 at a time
-          const uint64_t a_p = umma_smem_desc(sP + kk * 16 * 128, kAttTile * 128, 8 * 128, l128);
-          const uint64_t a_ds = umma_smem_desc(sDS + kk * 16 * 128, kAttTile * 128, 8 * 128, l128);
-          const uint64_t b_do = umma_smem_desc(sDO + st * kQBytes + kk * 16 * (kAttD * 2), kQBytes, 8 * (kAttD * 2), l64);
-          const uint64_t b_q = umma_smem_desc(sQ + st * kQBytes + kk * 16 * (kAttD * 2), kQBytes, 8 * (kAttD * 2), l64);
-          umma_f16(tmem_dv, a_p, b_do, idesc_t, (i | kk) != 0 ? 1u : 0u);
-          umma_f16(tmem_dk, a_ds, b_q, idesc_t, (i | kk) != 0 ? 1u : 0u);
+          const uint64_t a_p = gmma_desc(sP + g * (kAttTile * 128) + kk * 16 * 128, kAttTile * 128, 8 * 128, l128);
+          const uint64_t a_ds = gmma_desc(sDS + g * (kAttTile * 128) + kk * 16 * 128, kAttTile * 128, 8 * 128, l128);
+          const uint64_t b_do = gmma_desc(sDO + st * kQBytes + kk * 16 * (kAttD * 2), kQBytes, 8 * (kAttD * 2), l64);
+          const uint64_t b_q = gmma_desc(sQ + st * kQBytes + kk * 16 * (kAttD * 2), kQBytes, 8 * (kAttD * 2), l64);
+          Wgmma<kAttD>::mma<1, 1>(dv[g], a_p, b_do, 1u);
+          Wgmma<kAttD>::mma<1, 1>(dk[g], a_ds, b_q, 1u);
         }
-        umma_commit(bar_done);
-        umma_commit(bar_empty + 8 * st);
-      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operand(dv[0]); wgmma_fence_operand(dv[1]);
+      wgmma_fence_operand(dk[0]); wgmma_fence_operand(dk[1]);
+      if (t == 0) mbar_arrive(bar_empty + 8 * st);
     }
-  } else {
-    const int quad = warp & 3, row = quad * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(quad * 32) << 16;
-    for (int i = 0; i < ntiles; ++i) {
-      const int qi = i * kAttTile + row;
-      const size_t stat = (static_cast<size_t>(b) * p.heads + h) * p.lq + qi;
-      float lse_log2 = qi < p.lq ? p.lse[stat] * 1.4426950408889634f : INFINITY;  // rows beyond lq: p = 0
-      if (lse_log2 == -INFINITY) lse_log2 = INFINITY;                                 // fully masked query: zero gradients instead of NaN
-      const float dsum = qi < p.lq ? p.dsum[stat] : 0.f;
-      mbar_wait(bar_sdp, i & 1);
-      tc_fence_after();
-      if (i > 0) mbar_wait(bar_done, (i - 1) & 1);  // the previous tile's P / dS have been consumed
-      uint32_t drop_key = 0;
-      if constexpr (DROP) drop_key = drop_row_key(p.drop.seed, static_cast<uint32_t>(b * p.heads + h), static_cast<uint32_t>(qi));
-#pragma unroll 1
-      for (int c = 0; c < kAttTile; c += 32)
-        bwd_chunk<DROP>(tmem_s, tmem_dp, lane_base, c, row, s_bias, lse_log2, dsum, p.scale, p.scale_log2, sP, sDS, true, p.drop, drop_key, k0);
-      fence_proxy_async();
-      tc_fence_before();
-      mbar_arrive(bar_pds);
-    }
-    mbar_wait(bar_done, (ntiles - 1) & 1);
-    tc_fence_after();
-    const int key = k0 + row;  // accumulator row = key index
-    uint32_t o[32];
-    tmem_ld_32x32(tmem_dv + lane_base, o);
-    tmem_ld_wait();
+    const int key = k0 + t;  // accumulator row = key index
+    float o[32];
+    acc_row32(dv, stS, t, o);
     if (key < p.lk) store_row32(p.dv + (static_cast<size_t>(b) * p.lk + key) * p.dv_pitch + p.dv_coff + h * kAttD, o);
-    tmem_ld_32x32(tmem_dk + lane_base, o);
-    tmem_ld_wait();
+    acc_row32(dk, stS, t, o);
     if (key < p.lk) store_row32(p.dk + (static_cast<size_t>(b) * p.lk + key) * p.dk_pitch + p.dk_coff + h * kAttD, o);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<512>(s_tmem);
 }
 
 template <bool DROP>
-__global__ void __launch_bounds__(kAttThreads)
+__global__ void __launch_bounds__(kAttThreads, 1)
 attention_bwd_q_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                        const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ AttnBwdParams p) {
   pdl_sync();
   extern __shared__ uint8_t smem_dyn[];
-  __shared__ __align__(8) uint64_t s_bar[8];  // qdo_full, kv_full[2], kv_empty[2], sdp_full, ds_ready, mma_done
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t s_bar[5];  // qdo_full, kv_full[2], kv_empty[2]
   __shared__ __align__(16) float s_bias[2][kAttTile];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = warp_id_uniform();
   const int q0 = blockIdx.x * kAttTile, h = blockIdx.y, b = blockIdx.z;
   const uint32_t base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
   const uint32_t sQ = base, sDO = sQ + kQBytes, sK = sDO + kQBytes, sV = sK + 2 * kKVBytes, sDS = sV + 2 * kKVBytes;
+  float* const stS = reinterpret_cast<float*>(smem_dyn + (sDS + kPBytes - smem_u32(smem_dyn)));
+  float* const stDP = stS + 64 * kSPitch;
   const uint32_t bar_q = smem_u32(&s_bar[0]), bar_full = smem_u32(&s_bar[1]), bar_empty = smem_u32(&s_bar[3]);
-  const uint32_t bar_sdp = smem_u32(&s_bar[5]), bar_ds = smem_u32(&s_bar[6]), bar_done = smem_u32(&s_bar[7]);
   const int ntiles = (p.lk + kAttTile - 1) / kAttTile;
 
   if (threadIdx.x == 0) {
@@ -505,18 +503,11 @@ attention_bwd_q_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
       mbar_init(bar_full + 8 * s, 1);
       mbar_init(bar_empty + 8 * s, 1);
     }
-    mbar_init(bar_sdp, 1);
-    mbar_init(bar_ds, kAttTile);
-    mbar_init(bar_done, 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc<512>(smem_u32(&s_tmem));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_s = s_tmem, tmem_dp = s_tmem + 128, tmem_dq = s_tmem + 256;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (elect_one()) {
       mbar_expect_tx(bar_q, 2 * kQBytes);
       tma_load_5d(sQ, &tmQ, bar_q, p.q_coff + h * kAttD, q0, 0, 0, b);
@@ -529,71 +520,67 @@ attention_bwd_q_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         tma_load_5d(sV + st * kKVBytes, &tmV, bar_full + 8 * st, p.v_coff + h * kAttD, j * kAttTile, 0, 0, b);
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      const uint32_t idesc_s = umma_idesc_bf16(128, 128, 0, 0);
-      const uint32_t idesc_q = umma_idesc_bf16(128, kAttD, 0, 1);  // A = dS (K-major), B = K tile (MN-major): as P V in the forward kernel
-      const uint32_t l64 = umma_layout_code(64), l128 = umma_layout_code(128);
-      mbar_wait(bar_q, 0);
-      for (int j = 0; j < ntiles; ++j) {
-        const int st = j & 1;
-        mbar_wait(bar_full + 8 * st, (j >> 1) & 1);
-        tc_fence_after();
+  } else if (warp < 4) {
+    const int t = threadIdx.x, tid = t;
+    const int rl = t & 63, cbeg = (t >> 6) * 64;  // staged row of this thread and the 64 columns of it that it converts
+    const uint32_t l64 = gmma_layout_code(64), l128 = gmma_layout_code(128);
+    // per-row terms of the two query rows this thread converts (rows rl and 64 + rl of the tile)
+    float lse_log2[2], dsum[2];
+    uint32_t drop_key[2] = {0u, 0u};
 #pragma unroll
-        for (int k = 0; k < kAttD / 16; ++k) {
-          umma_f16(tmem_s, umma_smem_desc(sQ + k * 32, 16, 512, l64), umma_smem_desc(sK + st * kKVBytes + k * 32, 16, 512, l64), idesc_s, k != 0 ? 1u : 0u);
-          umma_f16(tmem_dp, umma_smem_desc(sDO + k * 32, 16, 512, l64), umma_smem_desc(sV + st * kKVBytes + k * 32, 16, 512, l64), idesc_s, k != 0 ? 1u : 0u);
-        }
-        umma_commit(bar_sdp);
-        mbar_wait(bar_ds, j & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < kAttTile / 16; ++kk) {
-          const uint64_t da = umma_smem_desc(sDS + (kk >> 2) * (kAttTile * 128) + (kk & 3) * 32, 16, 1024, l128);
-          const uint64_t db = umma_smem_desc(sK + st * kKVBytes + kk * 16 * (kAttD * 2), kKVBytes, 8 * (kAttD * 2), l64);
-          umma_f16(tmem_dq, da, db, idesc_q, (j | kk) != 0 ? 1u : 0u);
-        }
-        umma_commit(bar_done);
-        umma_commit(bar_empty + 8 * st);
-      }
+    for (int hf = 0; hf < 2; ++hf) {
+      const int qi = q0 + 64 * hf + rl;
+      const size_t stat = (static_cast<size_t>(b) * p.heads + h) * p.lq + qi;
+      lse_log2[hf] = qi < p.lq ? p.lse[stat] * 1.4426950408889634f : INFINITY;
+      if (lse_log2[hf] == -INFINITY) lse_log2[hf] = INFINITY;
+      dsum[hf] = qi < p.lq ? p.dsum[stat] : 0.f;
+      if constexpr (DROP) drop_key[hf] = drop_row_key(p.drop.seed, static_cast<uint32_t>(b * p.heads + h), static_cast<uint32_t>(qi));
     }
-  } else {
-    const int quad = warp & 3, row = quad * 32 + lane, tid = threadIdx.x - 64;
-    const uint32_t lane_base = static_cast<uint32_t>(quad * 32) << 16;
-    const int qi = q0 + row;
-    const size_t stat = (static_cast<size_t>(b) * p.heads + h) * p.lq + qi;
-    float lse_log2 = qi < p.lq ? p.lse[stat] * 1.4426950408889634f : INFINITY;
-    if (lse_log2 == -INFINITY) lse_log2 = INFINITY;
-    const float dsum = qi < p.lq ? p.dsum[stat] : 0.f;
-    uint32_t drop_key = 0;
-    if constexpr (DROP) drop_key = drop_row_key(p.drop.seed, static_cast<uint32_t>(b * p.heads + h), static_cast<uint32_t>(qi));
+    float dq[2][kAttD / 2];  // [query half]
+#pragma unroll
+    for (int g = 0; g < 2; ++g)
+#pragma unroll
+      for (int i = 0; i < kAttD / 2; ++i) dq[g][i] = 0.f;
+    mbar_wait(bar_q, 0);
     for (int j = 0; j < ntiles; ++j) {
+      const int st = j & 1;
       {
         const int key = j * kAttTile + tid;
         const bool dead = key >= p.lk || (p.mask != nullptr && p.mask[static_cast<size_t>(b) * p.lk + key] != 0);
         s_bias[j & 1][tid] = dead ? -INFINITY : 0.f;
       }
-      named_bar_sync(1, kAttTile);
-      mbar_wait(bar_sdp, j & 1);
-      tc_fence_after();
-      if (j > 0) mbar_wait(bar_done, (j - 1) & 1);
+      mbar_wait(bar_full + 8 * st, (j >> 1) & 1);
 #pragma unroll 1
-      for (int c = 0; c < kAttTile; c += 32)
-        bwd_chunk<DROP>(tmem_s, tmem_dp, lane_base, c, row, s_bias[j & 1], lse_log2, dsum, p.scale, p.scale_log2, sDS, sDS, false, p.drop, drop_key, j * kAttTile);
-      fence_proxy_async();
-      tc_fence_before();
-      mbar_arrive(bar_ds);
+      for (int hf = 0; hf < 2; ++hf) {
+        bwd_scores_half(sQ, sDO, sK + st * kKVBytes, sV + st * kKVBytes, hf, stS, stDP);
+        named_bar_sync(1, kAttTile);  // staged tiles (and, on the first half, the mask bias) complete
+#pragma unroll 1
+        for (int c = cbeg; c < cbeg + 64; c += 32)
+          bwd_chunk<DROP>(stS + rl * kSPitch, stDP + rl * kSPitch, c, 64 * hf + rl, s_bias[j & 1], lse_log2[hf], dsum[hf], p.scale, p.scale_log2, sDS, sDS,
+                          false, p.drop, drop_key[hf], j * kAttTile);
+        fence_proxy_async();
+        named_bar_sync(1, kAttTile);
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int g = 0; g < 2; ++g)
+#pragma unroll
+        for (int kk = 0; kk < kAttTile / 16; ++kk) {
+          const uint64_t da = gmma_desc(sDS + (kk >> 2) * (kAttTile * 128) + g * 64 * 128 + (kk & 3) * 32, 16, 1024, l128);
+          const uint64_t db = gmma_desc(sK + st * kKVBytes + kk * 16 * (kAttD * 2), kKVBytes, 8 * (kAttD * 2), l64);
+          Wgmma<kAttD>::mma<0, 1>(dq[g], da, db, 1u);  // A = dS (K-major), B = K tile (MN-major): as P V in the forward kernel
+        }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operand(dq[0]);
+      wgmma_fence_operand(dq[1]);
+      if (t == 0) mbar_arrive(bar_empty + 8 * st);
     }
-    mbar_wait(bar_done, (ntiles - 1) & 1);
-    tc_fence_after();
-    uint32_t o[32];
-    tmem_ld_32x32(tmem_dq + lane_base, o);
-    tmem_ld_wait();
+    const int qi = q0 + t;
+    float o[32];
+    acc_row32(dq, stS, t, o);
     if (qi < p.lq) store_row32(p.dq + (static_cast<size_t>(b) * p.lq + qi) * p.dq_pitch + p.dq_coff + h * kAttD, o);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<512>(s_tmem);
 }
 
 int check_seq(const yb200_act* a, const char* name) {

@@ -9,118 +9,22 @@
 
 namespace yb {
 
-static bool use_pair_kernel() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("YB200_CONV_PAIR");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-static bool use_v1_kernel() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("YB200_CONV_KERNEL");
-    v = (e && strcmp(e, "v1") == 0) ? 1 : 0;
-  }
-  return v == 1;
-}
-
 // ------------------------------------------------------------------------------------------------
 // kernel dispatch
 // ------------------------------------------------------------------------------------------------
-static bool use_staged_epilogue() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("YB200_CONV_STAGED");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
 template <int BN, int BK>
-static int launch_conv_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvGemmParams& p, dim3 grid, int stages,
-                            cudaStream_t st, const yb200_act* out_act) {
+static int launch_conv_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvGemmParams& p, dim3 grid, cudaStream_t st) {
   using Cfg = ConvGemmCfg<BN, BK>;
   const bool ext = p.epi_mode >= EPI_BF16_AFFINE;  // ConvNeXt / transformer epilogues live in their own instantiations
-  if constexpr (BN == 32 || BN == 64) {
-    // narrow column tiles: staged epilogue (swizzled smem tile -> TMA store, BatchNorm statistics on the tensor core)
-    const bool plain = (p.epi_mode == EPI_F16_STATS || p.epi_mode == EPI_F16 || p.epi_mode == EPI_BF16) && p.addend == nullptr && p.num_bnseg == 0;
-    if (use_staged_epilogue() && !use_v1_kernel() && plain && out_act != nullptr && p.cout % BN == 0 && p.out_mh == 1 && p.out_mw == 1 && p.out_sc == 1) {
-      const int m_tiles = grid.x, n_tiles = grid.y;
-      const int tw = 1 << p.log_tw, th = 1 << p.log_th, tn = 128 >> (p.log_tw + p.log_th);
-      CUtensorMap tmOut;
-      int rc = make_act_map(&tmOut, *out_act, false, BN, tw, th, tn);
-      if (rc) return rc;
-      const int fixed = 2 * 128 * BN * 2 + 2048;  // two staged tiles + the two constant ones operands
-      const int budget = 110 * 1024 - 1024 - fixed;
-      int slots_kb = budget / Cfg::kStageBytes;
-      const int num_kb = p.num_taps * p.cin_blocks;
-      int kbs = 1;
-      if (BK <= 32)
-        for (int t = 1; t <= num_kb; ++t)
-          if (num_kb % t == 0 && t * BK <= 144 && 2 * t <= slots_kb) kbs = t;
-      int pst = slots_kb / kbs;
-      if (pst > kMaxStagesP) pst = kMaxStagesP;
-      if (pst < 2) pst = 2;
-      const int smem = fixed + pst * kbs * Cfg::kStageBytes + 1024;
-      YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_staged_kernel<BN, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-      int groups = (2 * sm_count()) / n_tiles;
-      if (groups < 1) groups = 1;
-      if (groups > m_tiles) groups = m_tiles;
-      launch_k(conv_gemm_staged_kernel<BN, BK>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, tmOut, p, pst, kbs, n_tiles, m_tiles, out_act->c_off);
-      YB_CHECK_CUDA(cudaGetLastError());
-      return 0;
-    }
-  }
-  if (use_v1_kernel() && p.num_bnseg == 0) {  // one tile per CTA (kept for A/B comparison)
-    static PerDevice<int> max_set_dev(0);
-  int& max_set = max_set_dev.cur();
-    const int smem = stages * Cfg::kStageBytes + 1024;
-    if (smem > max_set) {
-      YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-      max_set = smem;
-    }
-    launch_k(conv_gemm_kernel<BN, BK>, grid, kConvThreads, smem, st, tmA, tmB, p, stages);
-    YB_CHECK_CUDA(cudaGetLastError());
-    return 0;
-  }
-  if constexpr (BN == 256) {
-    if (use_pair_kernel() && p.epi_mode != EPI_F32_BIAS && p.num_bnseg == 0 && p.num_phases == 0) {
-      // CTA pairs: 2 x 128 pixels x 256 channels per UMMA, one CTA per SM, 32 KB per stage and CTA at BLOCK_K 64
-      const int m_tiles = grid.x, n_tiles = grid.y;
-      constexpr int stage_bytes = 2 * 128 * BK * 2;
-      int pst = (212 * 1024) / stage_bytes;
-      if (pst > kMaxStagesP) pst = kMaxStagesP;
-      const int smem = pst * stage_bytes + 1024;
-      static PerDevice<int> max_set_pair_dev(0);
-  int& max_set_pair = max_set_pair_dev.cur();
-      if (smem > max_set_pair) {
-        YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_pair_kernel<BK, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_pair_kernel<BK, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        max_set_pair = smem;
-      }
-      const int pair_tiles = (m_tiles + 1) / 2;
-      int groups = (sm_count() / 2) / n_tiles;
-      if (groups < 1) groups = 1;
-      if (groups > pair_tiles) groups = pair_tiles;
-      if (ext)
-        launch_k(conv_gemm_pair_kernel<BK, true>, 2 * groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, p, pst, n_tiles, m_tiles);
-      else
-        launch_k(conv_gemm_pair_kernel<BK, false>, 2 * groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, p, pst, n_tiles, m_tiles);
-      YB_CHECK_CUDA(cudaGetLastError());
-      return 0;
-    }
-  }
-  // persistent kernel: two CTAs per SM (2 x 2 x BN TMEM columns <= 512; one CTA for BN = 256), ring as deep as the CTA's share
-  // of shared memory allows
+  // persistent kernel: one or two CTAs per SM as its launch bounds (conv_min_ctas); the ring is as deep as the CTA's share of shared
+  // memory allows after the epilogue staging tiles
   const int phases = p.num_phases == 4 ? 4 : 1;
   const int m_tiles = grid.x * phases, n_tiles = grid.y;  // work items of one column tile (pixel tiles x output-parity phases)
-  const int occ = BN == 256 ? 1 : 2;
+  const int occ = conv_min_ctas(BN, BK, p.num_bnseg > 0 ? 2 : 0);
   // fp32 rows with channel stride 1 and an odd pitch ([B, A, 85]): chunks go through a per-warp transpose scratch behind the ring
-  const bool xpose = p.epi_mode == EPI_F32_BIAS && p.out_sc == 1 && BN <= 128 && p.num_bnseg == 0;
-  const int budget = (occ == 1 ? 216 : 110) * 1024 - 1024 - (xpose ? kXposeBytes : 0);
+  const bool xpose = p.epi_mode == EPI_F32_BIAS && p.out_sc == 1 && p.num_bnseg == 0;
+  const int fixed = ConvEpiCfg<BN>::kStageBytes + (xpose ? kXposeBytes : 0);
+  const int budget = (occ == 1 ? 212 : 104) * 1024 - 1024 - fixed;
   int slots_kb = budget / Cfg::kStageBytes;  // k-blocks that fit in the ring
   // narrow layers (BLOCK_K 16 / 32) would spend their time on mbarrier round trips: put several k-blocks (up to 144
   // channels-taps) behind one barrier, keeping at least two ring slots
@@ -132,7 +36,7 @@ static int launch_conv_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
   int pst = slots_kb / kbs;
   if (pst > kMaxStagesP) pst = kMaxStagesP;
   if (pst < 2) pst = 2;
-  const int smem = pst * kbs * Cfg::kStageBytes + 1024 + (xpose ? kXposeBytes : 0);
+  const int smem = pst * kbs * Cfg::kStageBytes + 1024 + fixed;
   static PerDevice<int> max_set_p_dev(0);
   int& max_set_p = max_set_p_dev.cur();
   if (smem > max_set_p) {
@@ -145,14 +49,10 @@ static int launch_conv_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
   if (groups > m_tiles) groups = m_tiles;
   if (phases == 4 && groups > 1 && groups % 2 == 0) --groups;  // odd stride through the work items: every CTA cycles through all four phases (1 / 2 / 2 / 4 taps)
   if (p.num_bnseg > 0) {  // data gradient with fused BatchNorm-backward statistics
-    if constexpr (BN <= 128) {
-      YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_persistent_kernel<BN, BK, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-      launch_k(conv_gemm_persistent_kernel<BN, BK, 2>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, p, pst, kbs, n_tiles, m_tiles);
-      YB_CHECK_CUDA(cudaGetLastError());
-      return 0;
-    } else {
-      return fail(YB200_ERR_UNSUPPORTED, "fused BatchNorm-backward statistics need a column tile <= 128 (gradient tensors of < 256 channels)");
-    }
+    YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_persistent_kernel<BN, BK, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    launch_k(conv_gemm_persistent_kernel<BN, BK, 2>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, p, pst, kbs, n_tiles, m_tiles);
+    YB_CHECK_CUDA(cudaGetLastError());
+    return 0;
   }
   ConvGemmParams pp = p;
   pp.xpose = xpose ? 1 : 0;
@@ -164,39 +64,21 @@ static int launch_conv_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
   return 0;
 }
 
-static int launch_conv(int bn, int bk, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvGemmParams& p, dim3 grid,
-                       int stages, cudaStream_t st, const yb200_act* out_act = nullptr) {
+static int launch_conv(int bn, int bk, const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvGemmParams& p, dim3 grid, cudaStream_t st) {
 #define YB_CASE(BN, BK) \
-  if (bn == BN && bk == BK) return launch_conv_inst<BN, BK>(tmA, tmB, p, grid, stages, st, out_act);
+  if (bn == BN && bk == BK) return launch_conv_inst<BN, BK>(tmA, tmB, p, grid, st);
   YB_CASE(16, 16) YB_CASE(16, 32) YB_CASE(16, 64)
   YB_CASE(32, 16) YB_CASE(32, 32) YB_CASE(32, 64)
   YB_CASE(64, 16) YB_CASE(64, 32) YB_CASE(64, 64)
   YB_CASE(128, 16) YB_CASE(128, 32) YB_CASE(128, 64)
-  YB_CASE(256, 16) YB_CASE(256, 32) YB_CASE(256, 64)
 #undef YB_CASE
   return fail(YB200_ERR_UNSUPPORTED, "no conv_gemm instantiation for BLOCK_N=%d BLOCK_K=%d", bn, bk);
 }
 
-// pipeline depth: at most kMaxStages, never more than the K loop, and shallow enough that two CTAs fit in one SM's shared
-// memory (one CTA computes one tile: a second resident CTA hides its prologue / epilogue behind the other's MMAs)
-static int pick_stages(int bn, int bk, int num_kb) {
-  const int stage_bytes = (128 + bn) * bk * 2;
-  int st = num_kb < kMaxStages ? num_kb : kMaxStages;
-  while (st > 2 && 2 * (st * stage_bytes + 2048) > 227 * 1024) --st;
-  return st;
-}
 static int pick_block_k(int c) { return c % 64 == 0 ? 64 : (c % 32 == 0 ? 32 : (c % 16 == 0 ? 16 : 0)); }
-// 256-wide column tiles halve the activation (A operand) traffic per MMA: the 3x3 layers are L2-bandwidth bound at 128
-static int pick_block_n(int c) {
-  static int allow256 = -1;
-  if (allow256 < 0) {
-    const char* e = getenv("YB200_CONV_BN256");
-    allow256 = (e && e[0] == '0') ? 0 : 1;
-  }
-  if (c > 256 && c % 256 == 128) return 128;  // e.g. 384 = 3 x 128: no half-empty 256-wide tile
-  if (c >= 256 && allow256 && !use_v1_kernel()) return 256;
-  return c > 64 ? 128 : (c > 32 ? 64 : (c > 16 ? 32 : 16));
-}
+// column tiles up to 128: a 64 x 256 fp32 accumulator per consumer warpgroup (128 registers per thread) leaves too few registers for
+// the epilogue and spills
+static int pick_block_n(int c) { return c > 64 ? 128 : (c > 32 ? 64 : (c > 16 ? 32 : 16)); }
 
 static int check_act(const yb200_act* a, const char* name) {
   YB_REQUIRE(a != nullptr && a->ptr != nullptr, YB200_ERR_INVALID, "%s: null view", name);
@@ -372,9 +254,9 @@ extern "C" int yb200_pack_conv_weight_scaled(const float* w_oihw, const float* c
 // significant bits per plane: 16 bits with two planes, the full 24 of fp32 with three); plane j of an activation lives j * lo_delta channels
 // after plane 0 in the same NHWC buffer and the weight matrix is [rows][plane 0 taps | plane 1 taps | plane 2 taps].  The product keeps every
 // term x_i * w_j with i + j < planes (the dropped ones are below 2^-8planes relative) as extra taps of the SAME implicit GEMM -- one fp32
-// accumulator in TMEM, no extra kernel: 3 taps per spatial tap for two planes, 6 for three.
+// accumulator, no extra kernel: 3 taps per spatial tap for two planes, 6 for three.
 static int conv_fwd_common(const yb200_act* x, const void* w_fwd, int cout, int ksize, int stride, ConvGemmParams& p,
-                           cudaStream_t st, int lo_delta = 0, int planes = 1, const yb200_act* out_act = nullptr, int group = 0) {
+                           cudaStream_t st, int lo_delta = 0, int planes = 1, int group = 0) {
   YB_REQUIRE(w_fwd != nullptr, YB200_ERR_INVALID, "conv fwd: null weights");
   YB_REQUIRE((ksize == 1 && stride == 1) || (ksize == 2 && stride == 2) || (ksize == 3 && (stride == 1 || stride == 2)), YB200_ERR_UNSUPPORTED,
              "conv fwd: ksize=%d stride=%d not implemented", ksize, stride);
@@ -412,9 +294,9 @@ static int conv_fwd_common(const yb200_act* x, const void* w_fwd, int cout, int 
   if (group > 1 && ksize == 3 && stride == 1 && lo_delta == 0 && p.cin_blocks == 1 && x->c_off == 0 && x->c == x->c_pitch && (x->c / group) % 16 == 0) {
     // pixel-grouped 3x3 convolution (yb200_conv2d_fwd_fold): of the left neighbour GROUP only its last pixel reaches this group's outputs, of the
     // right neighbour only its first.  The side taps therefore load / multiply `cpp` channels instead of group * cpp: their activation box starts
-    // at the needed pixel (the rest of the box lies beyond the channel extent: TMA zero fill, no L2 traffic), the weight box at the matching
-    // columns, and the persistent kernel issues only the first cpp / 16 K steps.  Correct in every kernel variant (the skipped products are
-    // zero either way); YB200_STEM_SPARSE=0 keeps the dense taps for A/B runs.
+    // at the needed pixel (the rest of the box lies beyond the channel extent: TMA zero fill, no L2 traffic) and the weight box at the matching
+    // columns.  The products beyond the first cpp channels are zero either way (zero-filled activations on the left, zero weights of the
+    // expanded matrix on the right); YB200_STEM_SPARSE=0 keeps the dense taps for A/B runs.
     static int sparse = -1;
     if (sparse < 0) {
       const char* e = getenv("YB200_STEM_SPARSE");
@@ -423,21 +305,17 @@ static int conv_fwd_common(const yb200_act* x, const void* w_fwd, int cout, int 
     const int cpp = x->c / group;
     for (int t = 0; t < p.num_taps && sparse; ++t) {
       ConvTap& tp = p.taps[t];
-      if (tp.dw == -1) { tp.c0 += (group - 1) * cpp; tp.kb += (group - 1) * cpp; tp.ks = cpp / 16; }
-      if (tp.dw == 1) tp.ks = cpp / 16;
+      if (tp.dw == -1) { tp.c0 += (group - 1) * cpp; tp.kb += (group - 1) * cpp; }
     }
   }
   const int tw = 1 << p.log_tw, th = 1 << p.log_th, tn = 128 >> (p.log_tw + p.log_th);
   CUtensorMap tmA, tmB;
   int rc = make_act_map(&tmA, *x, stride == 2, bk, tw, th, tn);
   if (rc) return rc;
-  // the CTA-pair kernel (column tile 256) loads the weight tile as two 128-row halves, one per CTA
-  const bool pair = bn == 256 && use_pair_kernel() && !use_v1_kernel() && p.epi_mode != EPI_F32_BIAS;
-  rc = make_mat_map(&tmB, w_fwd, cout, kcols, pair ? 128 : bn, bk);
+  rc = make_mat_map(&tmB, w_fwd, cout, kcols, bn, bk);
   if (rc) return rc;
-  const int num_kb = p.num_taps * p.cin_blocks;
   dim3 grid(p.tiles_w * p.tiles_h * p.tiles_n, ceil_div(cout, bn));
-  return launch_conv(bn, bk, tmA, tmB, p, grid, pick_stages(bn, bk, num_kb), st, out_act);
+  return launch_conv(bn, bk, tmA, tmB, p, grid, st);
 }
 
 static int conv2d_fwd_impl(const yb200_act* x, const void* w_fwd, const yb200_act* z, int ksize, int stride, double* stat_sum, double* stat_sqsum,
@@ -470,7 +348,7 @@ static int conv2d_fwd_impl(const yb200_act* x, const void* w_fwd, const yb200_ac
   p.stat_sum = stat_sum;
   p.stat_sq = stat_sqsum;
   p.stat_fold = stat_fold;
-  return conv_fwd_common(x, w_fwd, z->c, ksize, stride, p, as_stream(stream), 0, 1, z, stat_fold > 0 ? z->c / stat_fold : 0);
+  return conv_fwd_common(x, w_fwd, z->c, ksize, stride, p, as_stream(stream), 0, 1, stat_fold > 0 ? z->c / stat_fold : 0);
 }
 
 extern "C" int yb200_conv2d_bn_silu_fwd(const yb200_act* x, const void* w_fwd, const float* scale, const float* shift,
@@ -591,7 +469,6 @@ extern "C" int yb200_conv1x1_nchw_f32_batched(const yb200_act* x, const void* w_
   set_tiles(p, x->n, x->h, x->w);
   YB_REQUIRE(p.log_tw + p.log_th == 7, YB200_ERR_UNSUPPORTED,
              "conv1x1_nchw_f32_batched: a 128-pixel tile would span images at %dx%d (use yb200_conv1x1_nchw_f32 per image)", x->h, x->w);
-  YB_REQUIRE(pick_block_n(cout) <= 128 && !use_v1_kernel(), YB200_ERR_UNSUPPORTED, "conv1x1_nchw_f32_batched: needs the persistent kernel");
   // conv_fwd_common, with the weight matrix map covering all images' rows
   const int bk = pick_block_k(x->c);
   YB_REQUIRE(bk != 0, YB200_ERR_UNSUPPORTED, "conv1x1_nchw_f32_batched: input channels %d must be a multiple of 16", x->c);
@@ -604,7 +481,7 @@ extern "C" int yb200_conv1x1_nchw_f32_batched(const yb200_act* x, const void* w_
   if ((rc = make_act_map(&tmA, *x, false, bk, tw, th, 1))) return rc;
   if ((rc = make_mat_map(&tmB, w_fwd, 1LL * x->n * cout, x->c, bn, bk))) return rc;
   dim3 grid(p.tiles_w * p.tiles_h * p.tiles_n, ceil_div(cout, bn));
-  return launch_conv(bn, bk, tmA, tmB, p, grid, pick_stages(bn, bk, p.cin_blocks), as_stream(stream));
+  return launch_conv(bn, bk, tmA, tmB, p, grid, as_stream(stream));
 }
 
 extern "C" int yb200_linear_gelu_fwd(const yb200_act* x, const void* w_fwd, const float* bias, const yb200_act* u_out, const yb200_act* h_out,
@@ -788,7 +665,7 @@ static int dgrad_impl(const yb200_act* dz, const void* w_dgrad, const yb200_act*
   const int tw = 1 << p.log_tw, th = 1 << p.log_th, tn = 128 >> (p.log_tw + p.log_th);
   CUtensorMap tmA, tmB;
   if ((rc = make_act_map(&tmA, *dz, false, bk, tw, th, tn))) return rc;
-  if ((rc = make_mat_map(&tmB, w_dgrad, cin, 1LL * taps_total * dz->c, (bn == 256 && use_pair_kernel() && !use_v1_kernel() && num_seg == 0) ? 128 : bn, bk))) return rc;
+  if ((rc = make_mat_map(&tmB, w_dgrad, cin, 1LL * taps_total * dz->c, bn, bk))) return rc;
   dim3 grid(p.tiles_w * p.tiles_h * p.tiles_n, ceil_div(cin, bn));
 
   if (stride == 1) {
@@ -801,7 +678,7 @@ static int dgrad_impl(const yb200_act* dz, const void* w_dgrad, const yb200_act*
         for (int kw = 0; kw < 3; ++kw) p.taps[nt++] = ConvTap{dz->c_off, 1 - kw, 0, 1 - kh, (kh * 3 + kw) * dz->c};
     }
     p.num_taps = nt;
-    return launch_conv(bn, bk, tmA, tmB, p, grid, pick_stages(bn, bk, nt * p.cin_blocks), st, (gelu_u == nullptr && addend == nullptr) ? dx : nullptr);
+    return launch_conv(bn, bk, tmA, tmB, p, grid, st);
   }
   // stride 2: input pixel (2i+ph, 2j+pw) receives  kh with (ph + 1 - kh) even:  ph=0 -> kh=1 (row i);  ph=1 -> kh=0 (row i+1), kh=2 (row i)
   auto phase_taps = [&](int ph, int pw, ConvTap* out) {
@@ -824,8 +701,7 @@ static int dgrad_impl(const yb200_act* dz, const void* w_dgrad, const yb200_act*
     const char* e = getenv("YB200_DGRAD_PHASES");
     one_launch = (e && e[0] == '4') ? 0 : 1;
   }
-  const bool pair = bn == 256 && use_pair_kernel() && num_seg == 0;  // the CTA-pair kernel keeps the per-phase launches
-  if (one_launch && !use_v1_kernel() && !pair) {
+  if (one_launch) {
     // all four phases in ONE persistent launch: the phases of a pixel tile run back to back on neighbouring CTAs and share its dz tile in L2
     int nt = 0;
     for (int ph = 0; ph < 2; ++ph)
@@ -836,14 +712,14 @@ static int dgrad_impl(const yb200_act* dz, const void* w_dgrad, const yb200_act*
     p.phase_tap[4] = nt;
     p.num_taps = nt;
     p.num_phases = 4;
-    return launch_conv(bn, bk, tmA, tmB, p, grid, pick_stages(bn, bk, p.cin_blocks), st);
+    return launch_conv(bn, bk, tmA, tmB, p, grid, st);
   }
   for (int ph = 0; ph < 2; ++ph)
     for (int pw = 0; pw < 2; ++pw) {
       const int nt = phase_taps(ph, pw, p.taps);
       p.num_taps = nt;
       p.out_ph = ph; p.out_pw = pw;
-      if ((rc = launch_conv(bn, bk, tmA, tmB, p, grid, pick_stages(bn, bk, nt * p.cin_blocks), st))) return rc;
+      if ((rc = launch_conv(bn, bk, tmA, tmB, p, grid, st))) return rc;
     }
   return 0;
 }
@@ -883,7 +759,6 @@ extern "C" int yb200_linear_dgrad_relu(const yb200_act* dz, const void* w_dgrad,
 namespace {
 struct WgradPlan {
   WgradParams p;
-  int tmem_cols;
   int splits;
   int smem;
   int tw, th, tn;
@@ -934,7 +809,8 @@ int plan_wgrad(const yb200_act* x, const yb200_act* dz, int ksize, int stride, W
       if (tp.dw == 1) tp.ks = cpp / 16;
     }
   }
-  p.tpc = p.num_taps == 1 ? 1 : 3;  // (9 taps per CTA for narrow layers was measured slower: many 2 KB TMA boxes per stage)
+  // taps per CTA: the accumulators of all of them live in registers (TPC * BN / 2 per thread), so 128-wide cin tiles take one tap each
+  p.tpc = (p.num_taps == 1 || p.bn == 128) ? 1 : 3;
   p.tap_groups = ceil_div(p.num_taps, p.tpc);
   p.dz_c0 = dz->c_off;
   choose_tile(dz->n, dz->h, dz->w, kWgPix, &p.log_tw, &p.log_th);
@@ -942,13 +818,10 @@ int plan_wgrad(const yb200_act* x, const yb200_act* dz, int ksize, int stride, W
   p.tiles_w = ceil_div(dz->w, pl->tw); p.tiles_h = ceil_div(dz->h, pl->th); p.tiles_n = ceil_div(dz->n, pl->tn);
   p.num_blocks = p.tiles_w * p.tiles_h * p.tiles_n;
   const int base = p.cout_tiles * p.cin_tiles * p.tap_groups;
-  int cols = p.tpc * p.bn;
-  int tc = 32;
-  while (tc < cols) tc <<= 1;
-  pl->tmem_cols = tc;
+  const int occ_regs = p.tpc * p.bn <= 96 ? 2 : 1;  // CTAs per SM the accumulator registers allow (wgrad_gemm_kernel launch bounds)
   const int stage = kWgPix * 2 * (p.kc_a * p.ma + p.kc_b * p.nb * p.tpc);
   p.stages = kWgStages;
-  if (std::min(512 / tc, (220 * 1024) / (stage * kWgStages + 1024)) <= 1) {  // one CTA per SM anyway: deepen the ring (YB200_WGRAD_STAGES caps it, A/B)
+  if (std::min(occ_regs, (220 * 1024) / (stage * kWgStages + 1024)) <= 1) {  // one CTA per SM anyway: deepen the ring (YB200_WGRAD_STAGES caps it, A/B)
     static int cap = -1;
     if (cap < 0) {
       const char* e = getenv("YB200_WGRAD_STAGES");
@@ -959,9 +832,9 @@ int plan_wgrad(const yb200_act* x, const yb200_act* dz, int ksize, int stride, W
     p.stages = std::max(kWgStages, std::min(cap, (220 * 1024 - 1024) / stage));
   }
   pl->smem = stage * p.stages + 1024;
-  // Split the pixel range so that ONE wave of CTAs covers the machine (every CTA pays TMEM allocation, pipeline fill and
-  // a full accumulator write-back, so extra waves are pure overhead); occupancy is bounded by TMEM columns and shared memory.
-  int occ = std::min(std::min(512 / tc, (220 * 1024) / pl->smem), 8);
+  // Split the pixel range so that ONE wave of CTAs covers the machine (every CTA pays pipeline fill and a full accumulator
+  // write-back, so extra waves are pure overhead); occupancy is bounded by registers and shared memory.
+  int occ = std::min(occ_regs, (220 * 1024) / pl->smem);
   if (occ < 1) occ = 1;
   int splits = (occ * sm_count()) / base;  // floor: a partial second wave would double the tail
   if (splits > p.num_blocks / 8) splits = p.num_blocks / 8;  // at least 8 pixel blocks per CTA
@@ -982,15 +855,15 @@ extern "C" int64_t yb200_conv2d_wgrad_workspace(const yb200_act* x, const yb200_
   return 4LL * pl.splits * pl.p.cout * pl.p.num_taps * pl.p.cin;
 }
 
-template <int TC>
+template <int BN, int TPC>
 static int launch_wgrad_inst(const CUtensorMap& tmDz, const CUtensorMap& tmX, const WgradPlan& pl, dim3 grid, cudaStream_t st) {
   static PerDevice<int> max_set_dev(0);
   int& max_set = max_set_dev.cur();
   if (pl.smem > max_set) {
-    YB_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<TC>, cudaFuncAttributeMaxDynamicSharedMemorySize, pl.smem));
+    YB_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BN, TPC>, cudaFuncAttributeMaxDynamicSharedMemorySize, pl.smem));
     max_set = pl.smem;
   }
-  launch_k_opt(use_pdl_wgrad(), wgrad_gemm_kernel<TC>, grid, kConvThreads, pl.smem, st, tmDz, tmX, pl.p);
+  launch_k_opt(use_pdl_wgrad(), wgrad_gemm_kernel<BN, TPC>, grid, kWgThreads, pl.smem, st, tmDz, tmX, pl.p);
   YB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1022,14 +895,15 @@ static int wgrad_impl(const yb200_act* x, const yb200_act* dz, int ksize, int st
   if ((rc = make_act_map(&tmDz, *dz, false, pl.p.kc_a, pl.tw, pl.th, pl.tn))) return rc;
   if ((rc = make_act_map(&tmX, *x, stride == 2, pl.p.kc_b, pl.tw, pl.th, pl.tn))) return rc;
   dim3 grid(pl.p.cout_tiles * pl.p.cin_tiles * pl.p.tap_groups, pl.splits);
-  switch (pl.tmem_cols) {
-    case 32: rc = launch_wgrad_inst<32>(tmDz, tmX, pl, grid, st); break;
-    case 64: rc = launch_wgrad_inst<64>(tmDz, tmX, pl, grid, st); break;
-    case 128: rc = launch_wgrad_inst<128>(tmDz, tmX, pl, grid, st); break;
-    case 256: rc = launch_wgrad_inst<256>(tmDz, tmX, pl, grid, st); break;
-    case 512: rc = launch_wgrad_inst<512>(tmDz, tmX, pl, grid, st); break;
-    default: return fail(YB200_ERR_UNSUPPORTED, "conv2d_wgrad: %d TMEM columns", pl.tmem_cols);
-  }
+  const int bn = pl.p.bn, tpc = pl.p.tpc;
+  if (bn == 16 && tpc == 1) rc = launch_wgrad_inst<16, 1>(tmDz, tmX, pl, grid, st);
+  else if (bn == 16 && tpc == 3) rc = launch_wgrad_inst<16, 3>(tmDz, tmX, pl, grid, st);
+  else if (bn == 32 && tpc == 1) rc = launch_wgrad_inst<32, 1>(tmDz, tmX, pl, grid, st);
+  else if (bn == 32 && tpc == 3) rc = launch_wgrad_inst<32, 3>(tmDz, tmX, pl, grid, st);
+  else if (bn == 64 && tpc == 1) rc = launch_wgrad_inst<64, 1>(tmDz, tmX, pl, grid, st);
+  else if (bn == 64 && tpc == 3) rc = launch_wgrad_inst<64, 3>(tmDz, tmX, pl, grid, st);
+  else if (bn == 128 && tpc == 1) rc = launch_wgrad_inst<128, 1>(tmDz, tmX, pl, grid, st);
+  else return fail(YB200_ERR_UNSUPPORTED, "conv2d_wgrad: no kernel for a %d-wide cin tile with %d taps per CTA", bn, tpc);
   if (rc) return rc;
   const long long total = 1LL * pl.p.cout * pl.p.num_taps * pl.p.cin;
   const int blocks = static_cast<int>(std::min<long long>((total + 31) / 32, 16 * sm_count()));

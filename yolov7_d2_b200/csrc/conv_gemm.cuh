@@ -1,25 +1,23 @@
-// Implicit-GEMM convolution on tcgen05 (sm_100a).
+// Implicit-GEMM convolution on wgmma (sm_90a).
 //
 //   D[128 pixels, BLOCK_N channels] = sum over (tap, cin-block)  A_tap[128 px, BLOCK_K] * B_tap[BLOCK_N, BLOCK_K]^T
 //
 // A is the NHWC bf16 activation tensor seen through a 5-D TMA map (c, w, p, h, n): a "tap" is a
 // coordinate offset of the 128-pixel box (TW x TH x TN), so zero padding is TMA out-of-bounds fill and
 // stride-2 convolutions are taps on the space-to-depth view (p = row parity, column parity folded into c).
-// B is the packed weight matrix [rows][taps*K] (K-major).  Accumulators live in TMEM; one CTA computes
-// one 128 x BLOCK_N output tile with a TMA->smem->UMMA mbarrier ring.
+// B is the packed weight matrix [rows][taps*K] (K-major).  Two consumer warpgroups hold the fp32 accumulators
+// of one 128 x BLOCK_N output tile in registers (64 rows each), fed by a TMA->smem mbarrier ring.
 //
 // Used for: conv forward (F3/F2/F8 of SURVEY.md par.8a), data-gradient (same kernel, transposed tap table)
 // and the 1x1 prediction convolutions (fp32 + bias epilogue).
 #pragma once
 #include <cuda_fp16.h>
 
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace yb {
 
-constexpr int kConvThreads = 192;  // warp 0: TMA producer, warp 1: TMEM alloc + MMA issuer, warps 2-5: epilogue
 constexpr int kMaxTaps = 54;  // 9 spatial taps x up to 6 operand-split terms (strict mode, conv_api.cu)
-constexpr int kMaxStages = 4;
 
 enum EpiMode : int {
   EPI_BF16 = 0,       // out = bf16(acc [+ addend])                          (data gradients)
@@ -137,10 +135,8 @@ struct ConvGemmCfg {
   static constexpr int kABytes = 128 * BLOCK_K * 2;
   static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTmemCols = BLOCK_N < 32 ? 32 : BLOCK_N;
-  static constexpr int kChunk = BLOCK_N < 32 ? 16 : 32;  // epilogue column chunk
   static_assert(BLOCK_K == 16 || BLOCK_K == 32 || BLOCK_K == 64, "BLOCK_K");
-  static_assert(BLOCK_N == 16 || BLOCK_N == 32 || BLOCK_N == 64 || BLOCK_N == 128 || BLOCK_N == 256, "BLOCK_N");
+  static_assert(BLOCK_N == 16 || BLOCK_N == 32 || BLOCK_N == 64 || BLOCK_N == 128, "BLOCK_N");
   static_assert(kABytes % (8 * kSwizzle) == 0 && kStageBytes % (8 * kSwizzle) == 0, "tiles must start on a swizzle-pattern boundary");
 };
 
@@ -165,9 +161,9 @@ __device__ __forceinline__ void store_bf16x8(__nv_bfloat16* dst, const float* v)
   *reinterpret_cast<uint4*>(dst) = u;
 }
 
-// One chunk (CH columns of one accumulator row per lane) of the epilogue, shared by all three kernels.
+// One chunk (CH columns of one accumulator row per lane) of the epilogue.
 //   part_sum / part_sq: this warp's shared-memory slots for the chunk's columns (EPI_F16_STATS); `accumulate` adds to them
-//   (persistent kernels: statistics over all tiles of the CTA) instead of overwriting.
+//   (statistics over all tiles of the CTA) instead of overwriting.
 // Per-column parameters (scale | shift / bias) of the CTA's column tile are staged in shared memory once per CTA; the epilogue reads
 // them with 16-byte broadcast loads (per-element __ldg plus a null test per element made the parameterised epilogues 2-3x slower
 // than the plain one).  Columns beyond cout hold (1, 0).
@@ -213,21 +209,8 @@ __device__ __forceinline__ void load_z_chunk(const __half* zrow, bool valid, uin
   }
 }
 
-// The epilogue's per-element side input (GELU_BWD: the pre-activation u; otherwise the addend / residual) is a dependent global load in
-// a warp that has nothing else to do: the persistent kernels fetch it one chunk ahead (before the accumulator barrier for the first
-// chunk of a tile) so that its latency overlaps the TMEM load and the arithmetic of the previous chunk.
-template <int CH>
-__device__ __forceinline__ void load_side_chunk(const __nv_bfloat16* side_row, bool valid, int cbase, int cout, uint4 (&dst)[CH / 8]) {
-#pragma unroll
-  for (int k = 0; k < CH / 8; ++k) {
-    dst[k] = make_uint4(0u, 0u, 0u, 0u);
-    if (valid && cbase + 8 * k < cout) dst[k] = *reinterpret_cast<const uint4*>(side_row + cbase + 8 * k);
-  }
-}
-
 // EXT = false: the YOLOX training / inference modes only (EPI_BF16 .. EPI_BF16_BN_SILU); EXT = true adds the ConvNeXt / transformer
-// modes and the prefetched side input.  Two instantiations per kernel keep the hot YOLOX kernels as small as they were before the
-// extra modes existed (the combined epilogue cost the 3x3 kernels 2-13 % through registers and code size).
+// modes.  Two instantiations per kernel keep the hot YOLOX kernels free of the extra modes' registers and code.
 // fp32 rows with a pitch that is not a multiple of 16 bytes (the [B, A, 85] prediction tensor): a lane-per-pixel store touches 32 different
 // sectors per instruction.  With the per-warp scratch each store instruction writes 32 consecutive floats of ONE pixel row instead.
 constexpr int kXposeWarpFloats = 32 * 33 + 64;              // 32 x 32 chunk (pitch 33: conflict free both ways) + 32 row offsets (8 B each)
@@ -236,7 +219,7 @@ constexpr int kXposeBytes = 8 * kXposeWarpFloats * 4;       // eight epilogue wa
 template <int CH, bool EXT = true>
 __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, float (&v)[CH], bool valid, long long pix_off, long long add_off,
                                                     int cbase, int lane, float* part_sum, float* part_sq, bool accumulate,
-                                                    const float* col_scale, const float* col_shift, const uint4* side = nullptr,
+                                                    const float* col_scale, const float* col_shift,
                                                     const uint4* zq = nullptr, float* xp = nullptr) {
   if (p.epi_mode == EPI_F32_BIAS) {
     if (xp != nullptr) {
@@ -305,7 +288,7 @@ __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, flo
   #pragma unroll
       for (int i = 0; i < CH; i += 8) {
         if (cbase + i < p.cout) {
-          const uint4 u = side ? side[i >> 3] : *reinterpret_cast<const uint4*>(a + i);
+          const uint4 u = *reinterpret_cast<const uint4*>(a + i);
           // bf16 sign / zero test on the raw bits: positive and non-zero
           v[i + 0] = (u.x & 0xFFFFu) - 1u < 0x7FFFu ? v[i + 0] : 0.f; v[i + 1] = (u.x >> 16) - 1u < 0x7FFFu ? v[i + 1] : 0.f;
           v[i + 2] = (u.y & 0xFFFFu) - 1u < 0x7FFFu ? v[i + 2] : 0.f; v[i + 3] = (u.y >> 16) - 1u < 0x7FFFu ? v[i + 3] : 0.f;
@@ -335,7 +318,7 @@ __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, flo
   #pragma unroll
       for (int i = 0; i < CH; i += 8) {
         if (cbase + i < p.cout) {
-          const uint4 u = side ? side[i >> 3] : *reinterpret_cast<const uint4*>(a + i);
+          const uint4 u = *reinterpret_cast<const uint4*>(a + i);
           v[i + 0] *= gelu_erf_grad(bf16_lo(u.x)); v[i + 1] *= gelu_erf_grad(bf16_hi(u.x));
           v[i + 2] *= gelu_erf_grad(bf16_lo(u.y)); v[i + 3] *= gelu_erf_grad(bf16_hi(u.y));
           v[i + 4] *= gelu_erf_grad(bf16_lo(u.z)); v[i + 5] *= gelu_erf_grad(bf16_hi(u.z));
@@ -349,7 +332,7 @@ __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, flo
 #pragma unroll
     for (int i = 0; i < CH; i += 8) {
       if (cbase + i < p.cout) {
-        const uint4 u = (EXT && side && p.epi_mode != EPI_BF16_GELU_BWD && p.epi_mode != EPI_BF16_RELU_BWD) ? side[i >> 3] : *reinterpret_cast<const uint4*>(a + i);
+        const uint4 u = *reinterpret_cast<const uint4*>(a + i);
         v[i + 0] += bf16_lo(u.x); v[i + 1] += bf16_hi(u.x);
         v[i + 2] += bf16_lo(u.y); v[i + 3] += bf16_hi(u.y);
         v[i + 4] += bf16_lo(u.z); v[i + 5] += bf16_hi(u.z);
@@ -448,180 +431,57 @@ __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, flo
   }
 }
 
-template <int BLOCK_N, int BLOCK_K>
-__global__ void __launch_bounds__(kConvThreads)
-conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ ConvGemmParams p, int num_stages) {
-  pdl_sync();
-  using Cfg = ConvGemmCfg<BLOCK_N, BLOCK_K>;
-  extern __shared__ uint8_t smem_dyn[];
-  __shared__ __align__(8) uint64_t s_bar[2 * kMaxStages + 1];
-  __shared__ uint32_t s_tmem;
-  __shared__ float s_part[4][2][BLOCK_N];  // per epilogue warp: column sums / sums of squares of its 32 rows
-  __shared__ __align__(16) float s_col[2][BLOCK_N];  // per-column scale | shift of this column tile
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;  // swizzled tiles need 1024B alignment
-  const uint32_t bar_full = smem_u32(&s_bar[0]);
-  const uint32_t bar_empty = smem_u32(&s_bar[kMaxStages]);
-  const uint32_t bar_acc = smem_u32(&s_bar[2 * kMaxStages]);
-
-  // tile coordinates
-  int t = blockIdx.x;
-  const int tw = t % p.tiles_w;
-  t /= p.tiles_w;
-  const int th = t % p.tiles_h;
-  const int tn = t / p.tiles_h;
-  const int log_tw = p.log_tw, log_th = p.log_th;
-  const int w0 = tw << log_tw, h0 = th << log_th, n0 = tn << (7 - log_tw - log_th);
-  const int col0 = blockIdx.y * BLOCK_N;
-  const int num_kb = p.num_taps * p.cin_blocks;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < num_stages; ++s) {
-      mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, 1);
-    }
-    mbar_init(bar_acc, 1);
-    mbar_fence_init();
-  }
-  stage_col_params<BLOCK_N>(p, col0, s_col);
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(smem_u32(&s_tmem));
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      tma_prefetch_desc(&tmA);
-      tma_prefetch_desc(&tmB);
-      int stage = 0;
-      uint32_t phase = 0;
-      int tap = 0, cb = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(bar_empty + 8 * stage, phase ^ 1u);
-        const uint32_t sa = smem_base + stage * Cfg::kStageBytes;
-        const uint32_t sb = sa + Cfg::kABytes;
-        const uint32_t full = bar_full + 8 * stage;
-        mbar_expect_tx(full, Cfg::kStageBytes);
-        const ConvTap& tp = p.taps[tap];
-        tma_load_5d(sa, &tmA, full, tp.c0 + cb * BLOCK_K, w0 + tp.dw, tp.p, h0 + tp.dh, n0);
-        tma_load_2d(sb, &tmB, full, tp.kb + cb * BLOCK_K, col0);
-        if (++cb == p.cin_blocks) { cb = 0; ++tap; }
-        if (++stage == num_stages) { stage = 0; phase ^= 1u; }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one elected thread) =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, BLOCK_N, 0, 0);
-      constexpr uint32_t lcode = umma_layout_code(Cfg::kSwizzle);
-      constexpr uint32_t sbo = 8 * Cfg::kSwizzle;  // 8 rows of one swizzle atom
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(bar_full + 8 * stage, phase);
-        tc_fence_after();
-        const uint32_t sa = smem_base + stage * Cfg::kStageBytes;
-        const uint32_t sb = sa + Cfg::kABytes;
-#pragma unroll
-        for (int k = 0; k < BLOCK_K / 16; ++k) {
-          const uint64_t da = umma_smem_desc(sa + k * 32, 16, sbo, lcode);
-          const uint64_t db = umma_smem_desc(sb + k * 32, 16, sbo, lcode);
-          umma_f16(tmem_base, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(bar_empty + 8 * stage);  // frees the smem slot when these MMAs retire
-        if (++stage == num_stages) { stage = 0; phase ^= 1u; }
-      }
-      umma_commit(bar_acc);  // accumulator complete
-    }
-  } else {
-    // ===================== epilogue: TMEM -> registers -> global =====================
-    const int q = warp & 3;  // TMEM lane quadrant this warp may access
-    const int m = q * 32 + lane;
-    const int xl = m & ((1 << log_tw) - 1);
-    const int yl = (m >> log_tw) & ((1 << log_th) - 1);
-    const int nl = m >> (log_tw + log_th);
-    const int x = w0 + xl, y = h0 + yl, n = n0 + nl;
-    const bool valid = (x < p.w_valid) && (y < p.h_valid) && (n < p.n_valid);
-    const long long pix_off = (long long)n * p.out_sn + (long long)(y * p.out_mh + p.out_ph) * p.out_sh +
-                              (long long)(x * p.out_mw + p.out_pw) * p.out_sw;
-    const long long add_off = (long long)n * p.add_sn + (long long)(y * p.out_mh + p.out_ph) * p.add_sh +
-                              (long long)(x * p.out_mw + p.out_pw) * p.add_sw;
-
-    mbar_wait(bar_acc, 0);
-    tc_fence_after();
-
-    constexpr int CH = Cfg::kChunk;
-#pragma unroll 1
-    for (int c = 0; c < BLOCK_N; c += CH) {
-      uint32_t r[CH];
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + c;
-      if constexpr (CH == 32) tmem_ld_32x32(taddr, r); else tmem_ld_32x16(taddr, r);
-      tmem_ld_wait();
-      float v[CH];
-#pragma unroll
-      for (int i = 0; i < CH; ++i) v[i] = __uint_as_float(r[i]);
-      const int cbase = col0 + c;
-      conv_epilogue_chunk<CH>(p, v, valid, pix_off, add_off, cbase, lane, &s_part[q][0][c], &s_part[q][1][c], false, &s_col[0][c], &s_col[1][c]);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-  if (epi_has_stats(p.epi_mode, p.stat_sum)) {
-    // one fp64 atomic per channel and CTA (after the block-wide barrier above: no named barrier, no shared atomics)
-    for (int e = threadIdx.x; e < BLOCK_N && col0 + e < p.cout; e += blockDim.x) {  // BLOCK_N may exceed the 192 threads
-      const float s1 = (s_part[0][0][e] + s_part[1][0][e]) + (s_part[2][0][e] + s_part[3][0][e]);
-      const float s2 = (s_part[0][1][e] + s_part[1][1][e]) + (s_part[2][1][e] + s_part[3][1][e]);
-      atomicAdd(p.stat_sum + col0 + e, static_cast<double>(s1));
-      if (p.stat_sq != nullptr) atomicAdd(p.stat_sq + col0 + e, static_cast<double>(s2));
-    }
-  }
-}
-
 // ================================================================================================
-// Persistent variant: each CTA walks a strided list of 128-pixel tiles for ONE column tile.  The TMA ring runs ahead across
-// tile boundaries, accumulators are double-buffered in TMEM (2 x BLOCK_N columns) so the epilogue of tile i overlaps the
-// MMAs of tile i+1, per-channel statistics are accumulated in shared memory over all tiles of the CTA (one fp64 atomic per
-// channel and CTA instead of per tile), and TMEM allocation / barrier setup / descriptor prefetch are paid once.
+// Persistent kernel: each CTA walks a strided list of 128-pixel tiles for ONE column tile.
+//   warps 0-3, 4-7  two consumer warpgroups.  Warpgroup g computes rows [64 g, 64 g + 64) of the tile with wgmma (accumulator in
+//                   registers) and then runs the epilogue of those rows: the accumulator passes through a per-warpgroup fp32 staging tile
+//                   in shared memory, kCols columns per round, so that every epilogue lane owns one pixel row, as conv_epilogue_chunk expects
+//   warp 8          TMA producer: the ring runs ahead across tile boundaries, so the loads of tile i+1 overlap the epilogue of tile i
+// Per-channel statistics are accumulated in shared memory over all tiles of the CTA (one fp64 atomic per channel and CTA instead of per
+// tile); barrier setup and descriptor prefetch are paid once.
 // grid.x = n_tiles * groups;  CTA b: column tile b % n_tiles, pixel tiles (b / n_tiles) + i * groups.
 // ================================================================================================
-constexpr int kMaxStagesP = 8;     // ring slots; one slot holds kb_per_slot consecutive k-blocks under a single mbarrier
-constexpr int kConvThreadsP = 320;  // warp 0 TMA, warp 1 MMA, warps 2-9 epilogue: two warps per TMEM lane quadrant, each
-                                    // draining half of the accumulator columns (memory-bound layers are epilogue-bound)
+constexpr int kMaxStagesP = 8;      // ring slots; one slot holds kb_per_slot consecutive k-blocks under a single mbarrier
+constexpr int kConvThreadsP = 288;  // two consumer warpgroups + one producer warp
+
+template <int BLOCK_N>
+struct ConvEpiCfg {
+  // accumulator columns staged per round: up to 32 at BN <= 64 (two CTAs per SM: 96 registers per thread), 64 above
+  static constexpr int kCols = BLOCK_N <= 64 ? (BLOCK_N < 32 ? BLOCK_N : 32) : 64;
+  static_assert(BLOCK_N % kCols == 0, "staging rounds must cover the column tile");
+  static constexpr int kPitch = kCols + 4;                    // floats per staged row: 16-byte aligned, conflict-free row reads
+  static constexpr int kHalves = BLOCK_N >= 32 ? 2 : 1;       // warps per 32-row quadrant, each taking kCols / kHalves columns of a round
+  static constexpr int kChunk = kCols / kHalves;              // 16 or 32 columns per conv_epilogue_chunk
+  static constexpr int kStageBytes = 2 * 64 * kPitch * 4;     // both warpgroups
+};
+
+__host__ __device__ constexpr int conv_min_ctas(int block_n, int block_k, int var) { return (block_n >= 128 || var == 2 || block_k == 16) ? 1 : 2; }
 
 // VAR: 0 = YOLOX training / inference epilogues, 1 = + ConvNeXt / transformer epilogues (EXT), 2 = data gradient with fused
 // BatchNorm-backward statistics (BnBwdSeg; epi_mode EPI_BF16)
 template <int BLOCK_N, int BLOCK_K, int VAR>
-__global__ void __launch_bounds__(kConvThreadsP, BLOCK_N == 256 ? 1 : 2)
+// two CTAs per SM (96 registers per thread: five of their 18 warps share one 16 K-register SM sub-partition) where that fits without
+// spilling; one CTA per SM (168 registers) for BN 128, for VAR 2 (the z loads) and for BLOCK_K 16 (the deep k-block slots); conv_min_ctas
+__global__ void __launch_bounds__(kConvThreadsP, conv_min_ctas(BLOCK_N, BLOCK_K, VAR))
 conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                             const __grid_constant__ ConvGemmParams p, int num_stages, int kb_per_slot, int n_tiles, int m_tiles) {
   using Cfg = ConvGemmCfg<BLOCK_N, BLOCK_K>;
+  using Epi = ConvEpiCfg<BLOCK_N>;
   constexpr bool EXT = VAR == 1;
   constexpr bool BNB = VAR == 2;
-  constexpr int kAccCols = Cfg::kTmemCols;          // columns of one accumulator
-  constexpr int kTmemAlloc = 2 * kAccCols;          // double buffered (power of two >= 64)
-  constexpr int kEpiHalves = BLOCK_N >= 32 ? 2 : 1; // column halves, one epilogue warp group (4 warps) each
-  constexpr int kHalfCols = BLOCK_N / kEpiHalves;
-  constexpr int CH = kHalfCols < 32 ? 16 : 32;      // columns per tcgen05.ld
+  constexpr int CH = Epi::kChunk;
   extern __shared__ uint8_t smem_dyn[];
-  __shared__ __align__(8) uint64_t s_bar[2 * kMaxStagesP + 4];
-  __shared__ uint32_t s_tmem;
+  __shared__ __align__(8) uint64_t s_bar[2 * kMaxStagesP];
   __shared__ float s_part[4][2][BLOCK_N];
   __shared__ __align__(16) float s_col[2][BLOCK_N];
 
-  const int warp = threadIdx.x >> 5;
+  const int warp = warp_id_uniform();
   const int lane = threadIdx.x & 31;
   const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
+  uint8_t* const smem_al = smem_dyn + (smem_base - smem_u32(smem_dyn));
+  const int ring_bytes = num_stages * kb_per_slot * Cfg::kStageBytes;
   const uint32_t bar_full = smem_u32(&s_bar[0]);
   const uint32_t bar_empty = smem_u32(&s_bar[kMaxStagesP]);
-  const uint32_t bar_acc_full = smem_u32(&s_bar[2 * kMaxStagesP]);       // [2]
-  const uint32_t bar_acc_empty = smem_u32(&s_bar[2 * kMaxStagesP + 2]);  // [2]
 
   const int n_tile = blockIdx.x % n_tiles;
   const int group = blockIdx.x / n_tiles;
@@ -632,25 +492,17 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
   if (threadIdx.x == 0) {
     for (int s = 0; s < num_stages; ++s) {
       mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(bar_acc_full + 8 * a, 1);
-      mbar_init(bar_acc_empty + 8 * a, 4 * kEpiHalves);  // one arrival per active epilogue warp
+      mbar_init(bar_empty + 8 * s, 2);  // one arrival per consumer warpgroup
     }
     mbar_fence_init();
   }
   for (int i = threadIdx.x; i < 4 * 2 * BLOCK_N; i += blockDim.x) (&s_part[0][0][0])[i] = 0.f;
-  if (warp == 1) tmem_alloc<kTmemAlloc>(smem_u32(&s_tmem));
-  pdl_sync();  // everything above touches only this CTA's shared / tensor memory: it overlaps the tail of the previous kernel
+  pdl_sync();  // everything above touches only this CTA's shared memory: it overlaps the tail of the previous kernel
   if constexpr (BNB) stage_col_params_bnseg<BLOCK_N>(p, col0, s_col);
   else stage_col_params<BLOCK_N>(p, col0, s_col);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (elect_one()) {
       tma_prefetch_desc(&tmA);
@@ -683,67 +535,56 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, BLOCK_N, 0, 0);
-      constexpr uint32_t lcode = umma_layout_code(Cfg::kSwizzle);
-      constexpr uint32_t sbo = 8 * Cfg::kSwizzle;
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int wi = group; wi < m_tiles; wi += groups, ++it) {
-        int m, tap0, ntaps, oph, opw;
-        conv_decode_work(p, wi, m, tap0, ntaps, oph, opw);
-        const int num_kb = ntaps * p.cin_blocks;
-        const int acc = it & 1;
-        mbar_wait(bar_acc_empty + 8 * acc, ((it >> 1) & 1) ^ 1u);  // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + acc * kAccCols;
-        int tap = tap0, cb = 0;
-        for (int kb = 0; kb < num_kb; kb += kb_per_slot) {
-          mbar_wait(bar_full + 8 * stage, phase);
-          tc_fence_after();
-          for (int j = 0; j < kb_per_slot; ++j) {
-            const uint32_t sa = smem_base + (stage * kb_per_slot + j) * Cfg::kStageBytes;
-            const uint32_t sb = sa + Cfg::kABytes;
-            const int ks = p.taps[tap].ks > 0 ? p.taps[tap].ks : BLOCK_K / 16;
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / 16; ++k) {
-              if (k < ks) {
-                const uint64_t da = umma_smem_desc(sa + k * 32, 16, sbo, lcode);
-                const uint64_t db = umma_smem_desc(sb + k * 32, 16, sbo, lcode);
-                umma_f16(tacc, da, db, idesc, (kb | j | k) != 0 ? 1u : 0u);
-              }
-            }
-            if (++cb == p.cin_blocks) { cb = 0; ++tap; }
-          }
-          umma_commit(bar_empty + 8 * stage);
-          if (++stage == num_stages) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(bar_acc_full + 8 * acc);
-      }
-    }
-  } else if ((warp - 2) / 4 < kEpiHalves) {
-    // ===================== epilogue =====================
-    const int q = warp & 3;              // TMEM lane quadrant (must be warp_id % 4)
-    const int half = (warp - 2) >> 2;    // which half of the columns this warp drains
-    const int cbeg = half * kHalfCols, cend = cbeg + kHalfCols;
-    // chunks that start at or beyond the last valid output channel are dead (cout not a multiple of the column tile): skip them
-    const int cend_live = min(cend, ((p.cout - col0 + CH - 1) / CH) * CH);
-    const bool side_is_aux = p.epi_mode == EPI_BF16_GELU_BWD || p.epi_mode == EPI_BF16_RELU_BWD;
-    const __nv_bfloat16* side_base = (EXT && BLOCK_N == 256) ? (side_is_aux ? p.aux_in : p.addend) : nullptr;  // narrower tiles run 2 CTAs / SM at 96 registers: no room
+  } else if (warp < 8) {
+    // ===================== consumer warpgroups: MMA, then the epilogue of their 64 rows =====================
+    const int g = warp >> 2;         // rows [64 g, 64 g + 64) of the tile
+    const int wl = warp & 3;
+    const int q = 2 * g + (wl & 1);  // 32-row quadrant whose epilogue this warp runs
+    const int half = wl >> 1;        // which part of each staged round of columns
     const int mrow = q * 32 + lane;
     const int xl = mrow & ((1 << log_tw) - 1);
     const int yl = (mrow >> log_tw) & ((1 << log_th) - 1);
     const int nl = mrow >> (log_tw + log_th);
+    float* const stg = reinterpret_cast<float*>(smem_al + ring_bytes) + g * 64 * Epi::kPitch;
     float* xp = nullptr;
-    if (!BNB && p.xpose)
-      xp = reinterpret_cast<float*>(smem_dyn + (smem_base - smem_u32(smem_dyn)) + num_stages * kb_per_slot * Cfg::kStageBytes) + (warp - 2) * kXposeWarpFloats;
-    int it = 0;
-    for (int wi = group; wi < m_tiles; wi += groups, ++it) {
-      int m, tap0, ntaps, oph, opw;
-      conv_decode_work(p, wi, m, tap0, ntaps, oph, opw);
+    if (!BNB && p.xpose) xp = reinterpret_cast<float*>(smem_al + ring_bytes + Epi::kStageBytes) + warp * kXposeWarpFloats;
+    constexpr uint32_t lcode = gmma_layout_code(Cfg::kSwizzle);
+    constexpr uint32_t sbo = 8 * Cfg::kSwizzle;  // 8 rows of one swizzle atom
+    float acc[BLOCK_N / 2];
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;  // defined on every path into the first wgmma (which overwrites it: scale-d 0)
+    wgmma_fence_operand(acc);
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int wi = group; wi < m_tiles; wi += groups) {
+      int m, tap, ntaps, oph, opw;
+      conv_decode_work(p, wi, m, tap, ntaps, oph, opw);
+      const int num_kb = ntaps * p.cin_blocks;
+      int j = 0, prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {  // one wgmma group per k-block; ring slots hold kb_per_slot of them
+        if (j == 0) mbar_wait(bar_full + 8 * stage, phase);
+        const uint32_t sa = smem_base + (stage * kb_per_slot + j) * Cfg::kStageBytes + g * 64 * Cfg::kSwizzle;
+        const uint32_t sb = smem_base + (stage * kb_per_slot + j) * Cfg::kStageBytes + Cfg::kABytes;
+        wgmma_fence_operand(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / 16; ++k)
+          Wgmma<BLOCK_N>::template mma<0, 0>(acc, gmma_desc(sa + k * 32, 16, sbo, lcode), gmma_desc(sb + k * 32, 16, sbo, lcode), (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs have completed
+        wgmma_fence_operand(acc);
+        // first k-block of a slot: every k-block of the previous slot has completed, hand that slot back to the producer
+        mbar_arrive_if(bar_empty + 8 * prev, j == 0 && prev >= 0 && (threadIdx.x & 127) == 0);
+        if (++j == kb_per_slot) {
+          j = 0;
+          prev = stage;
+          if (++stage == num_stages) { stage = 0; phase ^= 1u; }
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      mbar_arrive_if(bar_empty + 8 * prev, (threadIdx.x & 127) == 0);
+
       int t = m;
       const int tw = t % p.tiles_w;
       t /= p.tiles_w;
@@ -755,12 +596,6 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
                                 (long long)(x * p.out_mw + opw) * p.out_sw;
       const long long add_off = (long long)n * p.add_sn + (long long)(y * p.out_mh + oph) * p.add_sh +
                                 (long long)(x * p.out_mw + opw) * p.add_sw;
-      const int acc = it & 1;
-      const __nv_bfloat16* side_row = side_base ? side_base + (side_is_aux ? pix_off : add_off) : nullptr;
-      uint4 side[CH / 8];
-      if constexpr (EXT && BLOCK_N == 256) {
-        if (side_base != nullptr && cend_live > cbeg) load_side_chunk<CH>(side_row, valid, col0 + cbeg, p.cout, side);  // in flight during the barrier wait
-      }
       // fused BatchNorm-backward statistics: this pixel's row of z in each segment
       const __half* zrow[2] = {nullptr, nullptr};
       if constexpr (BNB) {
@@ -770,54 +605,44 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
             zrow[sg] = p.bnseg[sg].z + (long long)n * p.bnseg[sg].z_sn + (long long)(y * p.out_mh + oph) * p.bnseg[sg].z_sh +
                        (long long)(x * p.out_mw + opw) * p.bnseg[sg].z_sw - p.bnseg[sg].col_begin;
       }
-      mbar_wait(bar_acc_full + 8 * acc, (it >> 1) & 1);
-      tc_fence_after();
-      if (cend_live <= cbeg) {  // every column of this warp's share lies beyond cout: nothing to read
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_acc_empty + 8 * acc);
-        continue;
-      }
+      float* const r0 = stg + (16 * wl + (lane >> 2)) * Epi::kPitch + 2 * (lane & 3);  // this thread's fragment rows in the staging tile
+      float* const r1 = r0 + 8 * Epi::kPitch;
+      const float* const row_src = stg + ((wl & 1) * 32 + lane) * Epi::kPitch + half * CH;
 #pragma unroll 1
-      for (int c = cbeg; c < cend_live; c += CH) {
-        uint32_t r[CH];
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * kAccCols + c;
-        if constexpr (CH == 32) tmem_ld_32x32(taddr, r); else tmem_ld_32x16(taddr, r);
-        uint4 side_next[CH / 8];
-        const bool more = side_base != nullptr && c + CH < cend_live;
-        if constexpr (EXT && BLOCK_N == 256) {  // registers to spare (one CTA per SM): fetch the next chunk's side input before using this one
-          if (more) load_side_chunk<CH>(side_row, valid, col0 + c + CH, p.cout, side_next);
-        }
-        uint4 zq[CH / 8];
-        int zseg = -1;
-        if constexpr (BNB) {
-          zseg = bnseg_of(p, col0 + c);  // warp-uniform: chunks never straddle a segment boundary
-          if (zseg >= 0) load_z_chunk<CH>(zrow[zseg] + col0 + c, valid, zq);  // in flight while the accumulator chunk arrives
-        }
-        tmem_ld_wait();
-        if (c + CH >= cend_live) {  // this warp's last chunk is in registers: hand its share of the accumulator back
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_acc_empty + 8 * acc);
-        }
-        float v[CH];
+      for (int r = 0; r < BLOCK_N / Epi::kCols; ++r) {
+        named_bar_sync(1 + g, 128);  // every row of the previous round has been read
 #pragma unroll
-        for (int i = 0; i < CH; ++i) v[i] = __uint_as_float(r[i]);
-        const int cbase = col0 + c;
-        conv_epilogue_chunk<CH, EXT>(p, v, valid, pix_off, add_off, cbase, lane, &s_part[q][0][c], &s_part[q][1][c], true, &s_col[0][c], &s_col[1][c],
-                                (EXT && BLOCK_N == 256 && side_base) ? side : nullptr, (BNB && zseg >= 0) ? zq : nullptr, xp);
-        if constexpr (EXT && BLOCK_N == 256) {
-          if (more) {
-#pragma unroll
-            for (int k = 0; k < CH / 8; ++k) side[k] = side_next[k];
+        for (int i = 0; i < BLOCK_N / 8; ++i) {
+          if (i / (Epi::kCols / 8) == r) {
+            const int c = (i % (Epi::kCols / 8)) * 8;
+            *reinterpret_cast<float2*>(r0 + c) = make_float2(acc[4 * i], acc[4 * i + 1]);
+            *reinterpret_cast<float2*>(r1 + c) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
           }
+        }
+        named_bar_sync(1 + g, 128);
+        const int c = r * Epi::kCols + half * CH;  // tile column of this warp's chunk
+        // chunks at or beyond the last valid output channel are dead (cout not a multiple of the column tile)
+        if (half < Epi::kHalves && col0 + c < p.cout) {
+          float v[CH];
+#pragma unroll
+          for (int i = 0; i < CH; i += 4) {
+            const float4 f = *reinterpret_cast<const float4*>(row_src + i);
+            v[i] = f.x; v[i + 1] = f.y; v[i + 2] = f.z; v[i + 3] = f.w;
+          }
+          uint4 zq[CH / 8];
+          int zseg = -1;
+          if constexpr (BNB) {
+            zseg = bnseg_of(p, col0 + c);  // warp-uniform: chunks never straddle a segment boundary
+            if (zseg >= 0) load_z_chunk<CH>(zrow[zseg] + col0 + c, valid, zq);
+          }
+          conv_epilogue_chunk<CH, EXT>(p, v, valid, pix_off, add_off, col0 + c, lane, &s_part[q][0][c], &s_part[q][1][c], true, &s_col[0][c],
+                                       &s_col[1][c], (BNB && zseg >= 0) ? zq : nullptr, xp);
         }
       }
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) tmem_dealloc<kTmemAlloc>(tmem_base);
   if constexpr (BNB) {
     for (int e = threadIdx.x; e < BLOCK_N && col0 + e < p.cout; e += blockDim.x) {
       const int sg = bnseg_of(p, col0 + e);
@@ -830,466 +655,12 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
     return;
   }
   if (EXT ? epi_has_stats(p.epi_mode, p.stat_sum) : p.epi_mode == EPI_F16_STATS) {
-    for (int e = threadIdx.x; e < BLOCK_N && col0 + e < p.cout; e += blockDim.x) {  // BLOCK_N may exceed the 192 threads
+    for (int e = threadIdx.x; e < BLOCK_N && col0 + e < p.cout; e += blockDim.x) {  // BLOCK_N may exceed the thread count
       const float s1 = (s_part[0][0][e] + s_part[1][0][e]) + (s_part[2][0][e] + s_part[3][0][e]);
       const float s2 = (s_part[0][1][e] + s_part[1][1][e]) + (s_part[2][1][e] + s_part[3][1][e]);
       const int ch = p.stat_fold > 0 ? (col0 + e) % p.stat_fold : col0 + e;
       atomicAdd(p.stat_sum + ch, static_cast<double>(s1));
       if (p.stat_sq != nullptr) atomicAdd(p.stat_sq + ch, static_cast<double>(s2));
-    }
-  }
-}
-
-// ================================================================================================
-// Staged-epilogue variant for narrow column tiles (BLOCK_N = 32 / 64: the layers with the most pixels, where the classic epilogue is bound by
-// its own instruction count -- ncu: ~5 500 warp-instructions per 128 x 64 tile, half of them the shuffle butterflies of the BatchNorm statistics).
-//   * the accumulator chunk is packed to 16 bit and written ONCE to a swizzled shared-memory tile; one elected thread hands the tile to the TMA
-//     store unit (cp.async.bulk.tensor, coalesced full-line writes, hardware clipping of partial tiles);
-//   * the per-channel sums of BatchNorm (sum z, sum z^2) are computed by the TENSOR CORE from the same staged tile:
-//         S[., c] += ones[., 128 px] * Z[128 px, c]        (MN-major descriptor on the staged tile, as the weight-gradient kernel builds them)
-//     with a second staged tile of bf16 squares for sum z^2; the two accumulators live in TMEM next to the double-buffered output accumulators
-//     for the whole life of the CTA and are read once at the end.  ~100 instructions per warp and tile instead of ~700.
-// Modes: EPI_F16_STATS (forward training), EPI_F16 / EPI_BF16 without addend (no statistics: staged store only).  cout % BLOCK_N == 0.
-// ================================================================================================
-template <int BLOCK_N, int BLOCK_K>
-__global__ void __launch_bounds__(kConvThreadsP, 2)
-conv_gemm_staged_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
-                        const __grid_constant__ ConvGemmParams p, int num_stages, int kb_per_slot, int n_tiles, int m_tiles, int out_c0) {
-  using Cfg = ConvGemmCfg<BLOCK_N, BLOCK_K>;
-  static_assert(BLOCK_N == 32 || BLOCK_N == 64, "staged epilogue: column tiles of 32 or 64");
-  constexpr int kAccCols = BLOCK_N;                 // 32 or 64 (>= the 32-column allocation granule)
-  constexpr int kTmemAlloc = 4 * kAccCols;          // two output accumulators + sum + sum of squares
-  constexpr int kHalfCols = BLOCK_N / 2;            // two warps per TMEM lane quadrant, each draining half of the columns
-  constexpr int CH = kHalfCols;                     // 16 or 32 columns per tcgen05.ld
-  constexpr int kRowBytes = BLOCK_N * 2;            // 64 or 128: one pixel row of the staged tile = one swizzle span
-  constexpr int kTileBytes = 128 * kRowBytes;
-  constexpr int kEpiThreads = 256;
-  extern __shared__ uint8_t smem_dyn[];
-  __shared__ __align__(8) uint64_t s_bar[2 * kMaxStagesP + 5];
-  __shared__ uint32_t s_tmem;
-  __shared__ float s_stat[2][BLOCK_N];
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
-  // [staged Z tile][staged squares tile][ones fp16 1 KB][ones bf16 1 KB][operand ring ...]
-  const uint32_t s_z = smem_base, s_q = s_z + kTileBytes, s_one_h = s_q + kTileBytes, s_one_b = s_one_h + 1024;
-  const uint32_t ring_base = s_one_b + 1024;
-  const uint32_t bar_full = smem_u32(&s_bar[0]);
-  const uint32_t bar_empty = smem_u32(&s_bar[kMaxStagesP]);
-  const uint32_t bar_acc_full = smem_u32(&s_bar[2 * kMaxStagesP]);       // [2]
-  const uint32_t bar_acc_empty = smem_u32(&s_bar[2 * kMaxStagesP + 2]);  // [2]
-  const uint32_t bar_stage_free = smem_u32(&s_bar[2 * kMaxStagesP + 4]);
-
-  const bool stats = p.epi_mode == EPI_F16_STATS;
-  const bool f16 = p.epi_mode != EPI_BF16;
-  const int n_tile = blockIdx.x % n_tiles;
-  const int group = blockIdx.x / n_tiles;
-  const int groups = gridDim.x / n_tiles;
-  const int col0 = n_tile * BLOCK_N;
-  const int log_tw = p.log_tw, log_th = p.log_th;
-  const int num_kb = p.num_taps * p.cin_blocks;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < num_stages; ++s) {
-      mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(bar_acc_full + 8 * a, 1);
-      mbar_init(bar_acc_empty + 8 * a, 8);  // one arrival per epilogue warp
-    }
-    mbar_init(bar_stage_free, stats ? 2u : 1u);  // the issuing thread (TMA store has read the tile) [+ tcgen05.commit of the statistics MMAs]
-    mbar_fence_init();
-  }
-  // constant operand of the statistics MMAs: 8 rows x 128 B of 1.0 (every row group / box of the descriptor aliases these 1 KB)
-  for (int i = threadIdx.x; i < 512; i += blockDim.x) {
-    asm volatile("st.shared.u16 [%0], %1;" ::"r"(s_one_h + 2 * i), "h"(static_cast<unsigned short>(0x3C00)));
-    asm volatile("st.shared.u16 [%0], %1;" ::"r"(s_one_b + 2 * i), "h"(static_cast<unsigned short>(0x3F80)));
-  }
-  fence_proxy_async_smem();
-  if (warp == 1) tmem_alloc<kTmemAlloc>(smem_u32(&s_tmem));
-  pdl_sync();  // the set-up above touches only this CTA's shared / tensor memory: it overlaps the tail of the previous kernel
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
-  const uint32_t t_sum = tmem_base + 2 * kAccCols, t_sq = tmem_base + 3 * kAccCols;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      tma_prefetch_desc(&tmA);
-      tma_prefetch_desc(&tmB);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int m = group; m < m_tiles; m += groups) {
-        int t = m;
-        const int tw = t % p.tiles_w;
-        t /= p.tiles_w;
-        const int th = t % p.tiles_h;
-        const int tn = t / p.tiles_h;
-        const int w0 = tw << log_tw, h0 = th << log_th, n0 = tn << (7 - log_tw - log_th);
-        int tap = 0, cb = 0;
-        for (int kb = 0; kb < num_kb; kb += kb_per_slot) {
-          mbar_wait(bar_empty + 8 * stage, phase ^ 1u);
-          const uint32_t full = bar_full + 8 * stage;
-          mbar_expect_tx(full, Cfg::kStageBytes * kb_per_slot);
-          for (int j = 0; j < kb_per_slot; ++j) {
-            const uint32_t sa = ring_base + (stage * kb_per_slot + j) * Cfg::kStageBytes;
-            const ConvTap& tp = p.taps[tap];
-            tma_load_5d(sa, &tmA, full, tp.c0 + cb * BLOCK_K, w0 + tp.dw, tp.p, h0 + tp.dh, n0);
-            tma_load_2d(sa + Cfg::kABytes, &tmB, full, tp.kb + cb * BLOCK_K, col0);
-            if (++cb == p.cin_blocks) { cb = 0; ++tap; }
-          }
-          if (++stage == num_stages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, BLOCK_N, 0, 0);
-      constexpr uint32_t lcode = umma_layout_code(Cfg::kSwizzle);
-      constexpr uint32_t sbo = 8 * Cfg::kSwizzle;
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int m = group; m < m_tiles; m += groups, ++it) {
-        const int acc = it & 1;
-        mbar_wait(bar_acc_empty + 8 * acc, ((it >> 1) & 1) ^ 1u);
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + acc * kAccCols;
-        for (int kb = 0; kb < num_kb; kb += kb_per_slot) {
-          mbar_wait(bar_full + 8 * stage, phase);
-          tc_fence_after();
-          for (int j = 0; j < kb_per_slot; ++j) {
-            const uint32_t sa = ring_base + (stage * kb_per_slot + j) * Cfg::kStageBytes;
-            const uint32_t sb = sa + Cfg::kABytes;
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / 16; ++k) {
-              const uint64_t da = umma_smem_desc(sa + k * 32, 16, sbo, lcode);
-              const uint64_t db = umma_smem_desc(sb + k * 32, 16, sbo, lcode);
-              umma_f16(tacc, da, db, idesc, (kb | j | k) != 0 ? 1u : 0u);
-            }
-          }
-          umma_commit(bar_empty + 8 * stage);
-          if (++stage == num_stages) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(bar_acc_full + 8 * acc);
-      }
-    }
-  } else {
-    // ===================== epilogue: TMEM -> registers -> swizzled smem tile -> TMA store (+ statistics MMAs) =====================
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int cbeg = half * kHalfCols;
-    const int row = q * 32 + lane;
-    // 16-byte chunk c16 of row r lives at r * kRowBytes + ((c16 ^ f(r)) << 4): f(r) = r & 7 (128 B swizzle) or (r >> 1) & 3 (64 B swizzle)
-    const uint32_t row_off = static_cast<uint32_t>(row) * kRowBytes;
-    const uint32_t xr = kRowBytes == 128 ? static_cast<uint32_t>(row & 7) : static_cast<uint32_t>((row >> 1) & 3);
-    const bool issuer = warp == 2 && lane == 0;
-    constexpr uint32_t lcode_t = umma_layout_code(kRowBytes);
-    constexpr uint32_t lcode_one = umma_layout_code(128);
-    constexpr uint32_t idesc_h = umma_idesc_f16(128, BLOCK_N, 1, 1);
-    constexpr uint32_t idesc_b = umma_idesc_bf16(128, BLOCK_N, 1, 1);
-    int it = 0;
-    for (int m = group; m < m_tiles; m += groups, ++it) {
-      int t = m;
-      const int tw = t % p.tiles_w;
-      t /= p.tiles_w;
-      const int th = t % p.tiles_h;
-      const int tn = t / p.tiles_h;
-      const int acc = it & 1;
-      mbar_wait(bar_acc_full + 8 * acc, (it >> 1) & 1);
-      tc_fence_after();
-      uint32_t r[CH];
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * kAccCols + cbeg;
-      if constexpr (CH == 32) tmem_ld_32x32(taddr, r); else tmem_ld_32x16(taddr, r);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_acc_empty + 8 * acc);  // the accumulator is in registers: the next tile's MMAs may overwrite it
-      if (it > 0) mbar_wait(bar_stage_free, (it - 1) & 1);  // the previous tile has left the staging buffers
-      // rows of a partial tile that lie outside the pixel grid can carry non-zero accumulators (their taps reach valid input pixels): the TMA
-      // store clips them, the statistics must not see them
-      const int xg = (tw << log_tw) + (row & ((1 << log_tw) - 1)), yg = (th << log_th) + ((row >> log_tw) & ((1 << log_th) - 1));
-      const int ng = (tn << (7 - log_tw - log_th)) + (row >> (log_tw + log_th));
-      const bool valid = xg < p.w_valid && yg < p.h_valid && ng < p.n_valid;
-      uint32_t pk[CH / 2], pq[CH / 2];
-#pragma unroll
-      for (int i = 0; i < CH; i += 2) {
-        const float a = valid ? __uint_as_float(r[i]) : 0.f, b = valid ? __uint_as_float(r[i + 1]) : 0.f;
-        if (f16) {
-          pk[i >> 1] = pack_f16x2(a, b);
-          __half2 h;
-          *reinterpret_cast<uint32_t*>(&h) = pk[i >> 1];
-          const float2 f = __half22float2(h);      // squares of the STORED values
-          pq[i >> 1] = pack_bf16x2(f.x * f.x, f.y * f.y);
-        } else {
-          pk[i >> 1] = pack_bf16x2(a, b);
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < CH / 8; ++j) {
-        const uint32_t c16 = static_cast<uint32_t>(cbeg / 8 + j);
-        const uint32_t off = row_off + ((c16 ^ xr) << 4);
-        asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(s_z + off), "r"(pk[4 * j]), "r"(pk[4 * j + 1]), "r"(pk[4 * j + 2]), "r"(pk[4 * j + 3]) : "memory");
-        if (stats)
-          asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(s_q + off), "r"(pq[4 * j]), "r"(pq[4 * j + 1]), "r"(pq[4 * j + 2]), "r"(pq[4 * j + 3]) : "memory");
-      }
-      fence_proxy_async_smem();
-      named_bar_sync(1, kEpiThreads);
-      if (issuer) {
-        tc_fence_after();
-        const int w0 = tw << log_tw, h0 = th << log_th, n0 = tn << (7 - log_tw - log_th);
-        tma_store_5d(&tmOut, s_z, out_c0 + col0, w0, 0, h0, n0);
-        tma_store_commit();
-        if (stats) {
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {  // 128 pixels = 8 K-steps of 16
-            const uint64_t d1h = umma_smem_desc(s_one_h, 0, 0, lcode_one);
-            const uint64_t d1b = umma_smem_desc(s_one_b, 0, 0, lcode_one);
-            const uint64_t dz = umma_smem_desc(s_z + k * 16 * kRowBytes, 0, 8 * kRowBytes, lcode_t);
-            const uint64_t dq = umma_smem_desc(s_q + k * 16 * kRowBytes, 0, 8 * kRowBytes, lcode_t);
-            umma_f16(t_sum, d1h, dz, idesc_h, (it | k) != 0 ? 1u : 0u);
-            umma_f16(t_sq, d1b, dq, idesc_b, (it | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(bar_stage_free);
-        }
-        tma_store_wait_read();
-        mbar_arrive(bar_stage_free);
-      }
-    }
-    if (it > 0) mbar_wait(bar_stage_free, (it - 1) & 1);  // the last tile's statistics MMAs have completed
-    tc_fence_after();
-    if (issuer) tma_store_wait_all();
-    if (stats && it > 0 && warp == 4) {  // warp 4 owns TMEM lanes 0..31; every row of the statistics accumulators holds the column sums
-#pragma unroll 1
-      for (int c = 0; c < BLOCK_N; c += 32) {
-        uint32_t a[32], b[32];
-        tmem_ld_32x32(t_sum + c, a);
-        tmem_ld_32x32(t_sq + c, b);
-        tmem_ld_wait();
-        if (lane == 0) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) { s_stat[0][c + i] = __uint_as_float(a[i]); s_stat[1][c + i] = __uint_as_float(b[i]); }
-        }
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<kTmemAlloc>(tmem_base);
-  if (stats && group < m_tiles) {
-    for (int e = threadIdx.x; e < BLOCK_N && col0 + e < p.cout; e += blockDim.x) {
-      const int ch = p.stat_fold > 0 ? (col0 + e) % p.stat_fold : col0 + e;
-      atomicAdd(p.stat_sum + ch, static_cast<double>(s_stat[0][e]));
-      if (p.stat_sq != nullptr) atomicAdd(p.stat_sq + ch, static_cast<double>(s_stat[1][e]));
-    }
-  }
-}
-
-// ================================================================================================
-// CTA-pair variant (cta_group::2) for wide layers (column tile 256): the two CTAs of a cluster compute two consecutive
-// 128-pixel tiles as ONE 256 x 256 UMMA.  Each CTA loads its own activation tile and only HALF of the weight tile (the MMA
-// reads B from both CTAs' shared memory), which cuts the L2->SM operand traffic per MMA by a third -- the limiter of the
-// single-CTA kernel on the 3x3 layers (ncu: tensor pipe ~55 % active at 47 % L2 throughput).
-//   leader CTA (cluster rank 0): issues the MMAs; its full / acc_empty barriers collect both CTAs' arrivals
-//   both CTAs: TMA producer (signals the leader's full barrier), epilogue on their own TMEM half (= their own pixel tile)
-// grid.x = 2 * n_tiles * groups;  pair q = blockIdx.x / 2: column tile q % n_tiles, pixel-tile pairs (q / n_tiles) + i * groups.
-// ================================================================================================
-template <int BLOCK_K, bool EXT>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kConvThreadsP, 1)
-conv_gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                      const __grid_constant__ ConvGemmParams p, int num_stages, int n_tiles, int m_tiles) {
-  pdl_sync();
-  constexpr int BLOCK_N = 256;
-  constexpr int kSwizzle = BLOCK_K * 2;
-  constexpr int kABytes = 128 * BLOCK_K * 2;
-  constexpr int kBBytes = 128 * BLOCK_K * 2;          // this CTA's half of the 256-row weight tile
-  constexpr int kStageBytes = kABytes + kBBytes;
-  constexpr int kAccCols = 256, kTmemAlloc = 512;
-  constexpr int kHalfCols = 128, CH = 32;
-  extern __shared__ uint8_t smem_dyn[];
-  __shared__ __align__(8) uint64_t s_bar[2 * kMaxStagesP + 4];
-  __shared__ uint32_t s_tmem;
-  __shared__ float s_part[4][2][BLOCK_N];
-  __shared__ __align__(16) float s_col[2][BLOCK_N];
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
-  const uint32_t bar_full = smem_u32(&s_bar[0]);
-  const uint32_t bar_empty = smem_u32(&s_bar[kMaxStagesP]);
-  const uint32_t bar_acc_full = smem_u32(&s_bar[2 * kMaxStagesP]);
-  const uint32_t bar_acc_empty = smem_u32(&s_bar[2 * kMaxStagesP + 2]);
-
-  const int pair = blockIdx.x >> 1;
-  const int n_tile = pair % n_tiles;
-  const int group = pair / n_tiles;
-  const int groups = (gridDim.x >> 1) / n_tiles;
-  const int col0 = n_tile * BLOCK_N;
-  const int pair_tiles = (m_tiles + 1) >> 1;
-  const int log_tw = p.log_tw, log_th = p.log_th;
-  const int num_kb = p.num_taps * p.cin_blocks;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < num_stages; ++s) {
-      mbar_init(bar_full + 8 * s, 1);    // leader: its producer's arrive.expect_tx (bytes of BOTH CTAs)
-      mbar_init(bar_empty + 8 * s, 1);   // each CTA: multicast tcgen05.commit of the leader
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(bar_acc_full + 8 * a, 1);
-      mbar_init(bar_acc_empty + 8 * a, 16);  // leader: 8 epilogue warps of each CTA
-    }
-    mbar_fence_init();
-  }
-  for (int i = threadIdx.x; i < 4 * 2 * BLOCK_N; i += blockDim.x) (&s_part[0][0][0])[i] = 0.f;
-  stage_col_params<BLOCK_N>(p, col0, s_col);
-  if (warp == 1) tmem_alloc_pair<kTmemAlloc>(smem_u32(&s_tmem));
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();  // barriers of the peer are initialised before any remote arrive / TMA completion can reach them
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    if (elect_one()) {
-      tma_prefetch_desc(&tmA);
-      tma_prefetch_desc(&tmB);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int pt = group; pt < pair_tiles; pt += groups) {
-        int t = 2 * pt + static_cast<int>(rank);  // a tile index >= m_tiles lands entirely out of bounds: zero fill, masked epilogue
-        const int tw = t % p.tiles_w;
-        t /= p.tiles_w;
-        const int th = t % p.tiles_h;
-        const int tn = t / p.tiles_h;
-        const int w0 = tw << log_tw, h0 = th << log_th, n0 = tn << (7 - log_tw - log_th);
-        int tap = 0, cb = 0;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(bar_empty + 8 * stage, phase ^ 1u);
-          const uint32_t sa = smem_base + stage * kStageBytes;
-          const uint32_t full = bar_full + 8 * stage;
-          if (leader) mbar_expect_tx(full, 2 * kStageBytes);
-          const ConvTap& tp = p.taps[tap];
-          tma_load_5d_pair(sa, &tmA, full, tp.c0 + cb * BLOCK_K, w0 + tp.dw, tp.p, h0 + tp.dh, n0);
-          tma_load_2d_pair(sa + kABytes, &tmB, full, tp.kb + cb * BLOCK_K, col0 + static_cast<int>(rank) * 128);
-          if (++cb == p.cin_blocks) { cb = 0; ++tap; }
-          if (++stage == num_stages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (leader CTA only) =====================
-    if (leader && elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(256, BLOCK_N, 0, 0);
-      constexpr uint32_t lcode = umma_layout_code(kSwizzle);
-      constexpr uint32_t sbo = 8 * kSwizzle;
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int pt = group; pt < pair_tiles; pt += groups, ++it) {
-        const int acc = it & 1;
-        mbar_wait(bar_acc_empty + 8 * acc, ((it >> 1) & 1) ^ 1u);
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + acc * kAccCols;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(bar_full + 8 * stage, phase);
-          tc_fence_after();
-          const uint32_t sa = smem_base + stage * kStageBytes;
-          const uint32_t sb = sa + kABytes;
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / 16; ++k) {
-            const uint64_t da = umma_smem_desc(sa + k * 32, 16, sbo, lcode);
-            const uint64_t db = umma_smem_desc(sb + k * 32, 16, sbo, lcode);
-            umma_f16_pair(tacc, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit_pair(bar_empty + 8 * stage);  // frees the slot in both CTAs
-          if (++stage == num_stages) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit_pair(bar_acc_full + 8 * acc);   // both epilogues may drain
-      }
-    }
-  } else {
-    // ===================== epilogue (both CTAs, own TMEM = own pixel tile) =====================
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int cbeg = half * kHalfCols, cend = cbeg + kHalfCols;
-    // chunks that start at or beyond the last valid output channel are dead (cout not a multiple of the column tile): skip them
-    const int cend_live = min(cend, ((p.cout - col0 + CH - 1) / CH) * CH);
-    const bool side_is_aux = p.epi_mode == EPI_BF16_GELU_BWD || p.epi_mode == EPI_BF16_RELU_BWD;
-    const __nv_bfloat16* side_base = EXT ? (side_is_aux ? p.aux_in : p.addend) : nullptr;
-    const int mrow = q * 32 + lane;
-    const int xl = mrow & ((1 << log_tw) - 1);
-    const int yl = (mrow >> log_tw) & ((1 << log_th) - 1);
-    const int nl = mrow >> (log_tw + log_th);
-    int it = 0;
-    for (int pt = group; pt < pair_tiles; pt += groups, ++it) {
-      int t = 2 * pt + static_cast<int>(rank);
-      const int tw = t % p.tiles_w;
-      t /= p.tiles_w;
-      const int th = t % p.tiles_h;
-      const int tn = t / p.tiles_h;
-      const int x = (tw << log_tw) + xl, y = (th << log_th) + yl, n = (tn << (7 - log_tw - log_th)) + nl;
-      const bool valid = (x < p.w_valid) && (y < p.h_valid) && (n < p.n_valid);
-      const long long pix_off = (long long)n * p.out_sn + (long long)(y * p.out_mh + p.out_ph) * p.out_sh +
-                                (long long)(x * p.out_mw + p.out_pw) * p.out_sw;
-      const long long add_off = (long long)n * p.add_sn + (long long)(y * p.out_mh + p.out_ph) * p.add_sh +
-                                (long long)(x * p.out_mw + p.out_pw) * p.add_sw;
-      const int acc = it & 1;
-      const __nv_bfloat16* side_row = side_base ? side_base + (side_is_aux ? pix_off : add_off) : nullptr;
-      uint4 side[CH / 8];
-      if (side_base != nullptr && cend_live > cbeg) load_side_chunk<CH>(side_row, valid, col0 + cbeg, p.cout, side);  // in flight during the barrier wait
-      mbar_wait(bar_acc_full + 8 * acc, (it >> 1) & 1);
-      tc_fence_after();
-      if (cend_live <= cbeg) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive_leader(bar_acc_empty + 8 * acc);
-        continue;
-      }
-#pragma unroll 1
-      for (int c = cbeg; c < cend_live; c += CH) {
-        uint32_t r[CH];
-        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * kAccCols + c, r);
-        uint4 side_next[CH / 8];
-        const bool more = side_base != nullptr && c + CH < cend_live;
-        if (more) load_side_chunk<CH>(side_row, valid, col0 + c + CH, p.cout, side_next);
-        tmem_ld_wait();
-        if (c + CH >= cend_live) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_leader(bar_acc_empty + 8 * acc);
-        }
-        float v[CH];
-#pragma unroll
-        for (int i = 0; i < CH; ++i) v[i] = __uint_as_float(r[i]);
-        const int cbase = col0 + c;
-        conv_epilogue_chunk<CH, EXT>(p, v, valid, pix_off, add_off, cbase, lane, &s_part[q][0][c], &s_part[q][1][c], true, &s_col[0][c], &s_col[1][c],
-                                side_base ? side : nullptr);
-        if (more) {
-#pragma unroll
-          for (int k = 0; k < CH / 8; ++k) side[k] = side_next[k];
-        }
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync();  // neither CTA may free TMEM / exit while the peer's MMAs or remote arrives can still target it
-  if (warp == 1) tmem_dealloc_pair<kTmemAlloc>(tmem_base);
-  if (EXT ? epi_has_stats(p.epi_mode, p.stat_sum) : p.epi_mode == EPI_F16_STATS) {
-    for (int e = threadIdx.x; e < BLOCK_N && col0 + e < p.cout; e += blockDim.x) {
-      const float s1 = (s_part[0][0][e] + s_part[1][0][e]) + (s_part[2][0][e] + s_part[3][0][e]);
-      const float s2 = (s_part[0][1][e] + s_part[1][1][e]) + (s_part[2][1][e] + s_part[3][1][e]);
-      atomicAdd(p.stat_sum + col0 + e, static_cast<double>(s1));
-      if (p.stat_sq != nullptr) atomicAdd(p.stat_sq + col0 + e, static_cast<double>(s2));
     }
   }
 }

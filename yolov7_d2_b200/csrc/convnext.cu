@@ -7,7 +7,7 @@
 // These are HBM / CUDA-core bound streaming kernels: 16-byte or 8-byte accesses along the channel dimension, shared-memory halo
 // tiles for the 7x7 window, fixed-order reductions (bit-reproducible gradients).
 #include "host_common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include <algorithm>
 #include <type_traits>
 

@@ -6,7 +6,7 @@
 #include <cuda_fp16.h>
 
 #include "host_common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 using namespace yb;
 
@@ -86,7 +86,7 @@ int grid_for(long long work, int threads) {
 // ------------------------------------------------------------------------------------------------
 // preprocess: uint8 NCHW image batch -> Focus (space-to-depth) NHWC bf16 with 16 channels
 //   channel = patch*3 + rgb, patch order (top-left, bottom-left, top-right, bottom-right)   wrappers.py:210-220
-//   channels 12..15 are zero (pads K to the UMMA granule); pixels beyond (h_valid[n], w_valid[n]) read as pad_value
+//   channels 12..15 are zero (pads K to the MMA granule); pixels beyond (h_valid[n], w_valid[n]) read as pad_value
 //   (detectron2 ImageList.from_tensors with MODEL.PADDED_VALUE = 114, yolox.py:100-101).
 // ------------------------------------------------------------------------------------------------
 __global__ void preprocess_focus_kernel(const uint8_t* __restrict__ img, int n, int h, int w, const int* __restrict__ hw_valid,
@@ -203,7 +203,7 @@ bn_apply_silu_kernel(View z, View a, View res, View up, const float* __restrict_
   float s[8], t[8];
   if (fin.ssum != nullptr) {
     // one thread row derives the per-channel constants (fp64 only where the cancellation var = E[x^2] - mean^2 needs it; no fp64 division or
-    // square root: B200's fp64 pipe is narrow) and hands them to the other rows through shared memory
+    // square root: the fp64 pipe is narrow) and hands them to the other rows through shared memory
     __shared__ float s_st[2][kEwThreads * 8];
     if (threadIdx.y == 0) {
       const bool publish = blockIdx.x == 0;
@@ -800,8 +800,7 @@ static int bn_silu_bwd_impl(const yb200_act* z, const yb200_act* da, const yb200
   const int red_rows = red_shuffle ? static_cast<int>(block.x * block.y) / 32 : static_cast<int>(block.y);
   const size_t red_smem = static_cast<size_t>(red_rows) * 2 * z->c * sizeof(float);
   // tuning knob (tools/bench_bn.py): YB200_BN_RED = "U:MINB:ITERS" -- loads in flight per thread, resident blocks per SM, pixels per thread
-  static int red_u = -1, red_minb = 3, red_it = 0;  // U = 2 loads in flight, 3 blocks / SM: best INSIDE the step (17.21 vs 17.43 ms per step with 4 blocks / SM,
-                                                     // which wins the stand-alone sweep of profiles/r2_bn_backward_sweep.md by 4 %)
+  static int red_u = -1, red_minb = 3, red_it = 0;  // default U = 2 loads in flight, 3 blocks / SM
   if (red_u < 0) {
     red_u = 2;
     const char* e = getenv("YB200_BN_RED");

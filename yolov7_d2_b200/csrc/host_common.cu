@@ -31,7 +31,7 @@ bool use_pdl_wgrad() {
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("YB200_PDL_WGRAD");
-    v = (e && e[0] == '1') ? 1 : 0;  // default off: measured +1 % step throughput (profiles/r2_ab_runs.md)
+    v = (e && e[0] == '1') ? 1 : 0;  // default off: parked weight-gradient CTAs hold shared memory the main stream needs
   }
   return v == 1;
 }
@@ -46,7 +46,7 @@ int sm_count() {
   static int n[64] = {0};
   const int dev = current_device() & 63;
   if (n[dev] == 0) {
-    if (cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n[dev] <= 0) n[dev] = 148;
+    if (cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n[dev] <= 0) n[dev] = 132;
   }
   return n[dev];
 }

@@ -6,7 +6,7 @@
 // kernel text follows the reference formula line by line (including which epsilons are added where and the detached alpha
 // of CIoU).  Sub-gradients of min / max / clamp match torch: ties between the two arguments split 0.5 / 0.5.
 #include "host_common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 using namespace yb;
 

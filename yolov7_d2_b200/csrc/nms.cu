@@ -8,7 +8,7 @@
 #include <algorithm>
 
 #include "host_common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 using namespace yb;
 

@@ -7,7 +7,7 @@
 //   clip   FullModelGradientClippingOptimizer, optimizer/build.py:206-223 = clip_grad_norm_(all params, max_norm)
 // grad_scale folds the 1/world_size of the DDP mean into the same pass.
 #include "host_common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include <math.h>
 
 using namespace yb;

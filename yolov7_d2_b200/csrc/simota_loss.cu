@@ -10,7 +10,7 @@
 #include <algorithm>
 
 #include "host_common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 using namespace yb;
 

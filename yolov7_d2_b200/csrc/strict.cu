@@ -3,13 +3,13 @@
 //
 // Activations are stored as SPLIT bf16 planes: a = a0 + a1 [+ a2] with a0 = bf16(a), a1 = bf16(a - a0), a2 = bf16(a - a0 - a1) -- 16 significant
 // bits with two planes, all 24 bits of the fp32 value with three (the default) --, the planes `lo_delta` channels apart in one NHWC buffer, so every channel-slice view (torch.cat / Focus / upsample
-// fusions of the fast path) keeps working and the SAME tcgen05 implicit-GEMM kernel computes the partial products a_i * w_j (i + j < planes) into one fp32
-// TMEM accumulator (conv_api.cu: yb200_conv2d_fwd_split).  The pre-BatchNorm convolution output z stays in fp32.  The kernels here
+// fusions of the fast path) keeps working and the SAME wgmma implicit-GEMM kernel computes the partial products a_i * w_j (i + j < planes) into one fp32
+// accumulator (conv_api.cu: yb200_conv2d_fwd_split).  The pre-BatchNorm convolution output z stays in fp32.  The kernels here
 // are the element-wise stages around that GEMM; they are a verification mode, written for clarity, not for speed.
 #include <algorithm>
 
 #include "host_common.cuh"
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 using namespace yb;
 

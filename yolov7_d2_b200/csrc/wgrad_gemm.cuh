@@ -1,22 +1,22 @@
-// Weight-gradient GEMM on tcgen05 (sm_100a).
+// Weight-gradient GEMM on wgmma (sm_90a).
 //
 //   dW_tap[co, ci] = sum over pixels  dz[px, co] * x_tap[px, ci]
 //
 // Both operands are NHWC bf16 tensors, i.e. the contraction index (pixel) is the *slow* index of each
-// smem tile: UMMA "MN-major" descriptors.  dz tiles are dense 64-pixel boxes; x tiles are the same boxes
+// smem tile: "MN-major" descriptors for both wgmma operands.  dz tiles are dense 64-pixel boxes; x tiles are the same boxes
 // displaced by the tap (identical TMA maps / tap tables as the forward kernel), so zero padding and stride-2
-// need no extra code.  One CTA owns (cout tile of 128) x (cin tile of BN) x (tap group) x (pixel range) and keeps
-// one fp32 accumulator per tap in TMEM; partial tiles go to a split-K workspace reduced by wgrad_reduce_kernel
-// (deterministic, no atomics).
+// need no extra code.  One CTA owns (cout tile of 128) x (cin tile of BN) x (tap group) x (pixel range); two consumer warpgroups
+// (64 cout rows each) keep one fp32 accumulator per tap in registers; partial tiles go to a split-K workspace reduced by
+// wgrad_reduce_kernel (deterministic, no atomics).
 #pragma once
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include "conv_gemm.cuh"
 
 namespace yb {
 
-constexpr int kWgPix = 64;      // pixels per K block (4 UMMA K-steps)
-constexpr int kWgMaxTpc = 9;    // taps per CTA (9 when the cin tile is narrow enough for 9 accumulators in TMEM, else 3)
-constexpr int kWgStages = 3;     // default ring depth (keeps two or more CTAs per SM on the small layers)
+constexpr int kWgPix = 64;       // pixels per K block (4 wgmma K-steps)
+constexpr int kWgThreads = 288;  // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int kWgStages = 3;     // default ring depth (keeps two CTAs per SM on the small layers)
 constexpr int kWgMaxStages = 6;  // one-CTA-per-SM plans (the pixel-grouped stem: 40 KB stages) take as many as fit: the kernel is latency bound otherwise
 
 struct WgradParams {
@@ -34,26 +34,25 @@ struct WgradParams {
   int dz_c0;                      // channel offset of dz slice inside its buffer
   float* ws;                      // [split][cout][num_taps][cin] fp32
   ConvTap taps[kMaxTaps];         // x taps (c0, dw, p, dh).  ks > 0 (pixel-grouped stem, yb200_conv2d_wgrad_grouped): only the first 16 * ks channels
-                                  // of this tap's x box are real (the box starts at the one neighbour pixel that matters, the rest is TMA zero fill):
-                                  // the MMA runs with N = 16 * ks and the epilogue stores those columns at input channel kb, zeros elsewhere
+                                  // of this tap's x box matter (the box starts at the one neighbour pixel that does): the epilogue stores those
+                                  // accumulator columns at input channel kb (a multiple of 8), zeros elsewhere
 };
 
-template <int TMEM_COLS>
-__global__ void __launch_bounds__(kConvThreads)
+// one CTA-resident accumulator of 64 x BN fp32 per tap and warpgroup: TPC * BN / 2 registers per thread
+template <int BN, int TPC>
+__global__ void __launch_bounds__(kWgThreads, TPC * BN <= 96 ? 2 : 1)
 wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant__ CUtensorMap tmX,
                   const __grid_constant__ WgradParams p) {
   pdl_sync();
   extern __shared__ uint8_t smem_dyn[];
-  __shared__ __align__(8) uint64_t s_bar[2 * kWgMaxStages + 1];
+  __shared__ __align__(8) uint64_t s_bar[2 * kWgMaxStages];
   const int num_stages = p.stages;
-  __shared__ uint32_t s_tmem;
 
-  const int warp = threadIdx.x >> 5;
+  const int warp = warp_id_uniform();
   const int lane = threadIdx.x & 31;
   const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
   const uint32_t bar_full = smem_u32(&s_bar[0]);
   const uint32_t bar_empty = smem_u32(&s_bar[kWgMaxStages]);
-  const uint32_t bar_acc = smem_u32(&s_bar[2 * kWgMaxStages]);
 
   // work decomposition: blockIdx.x = ((cout_tile * cin_tiles + cin_tile) * tap_groups + group), blockIdx.y = split
   int w = blockIdx.x;
@@ -77,18 +76,13 @@ wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constan
   if (threadIdx.x == 0) {
     for (int s = 0; s < num_stages; ++s) {
       mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, 2);  // one arrival per consumer warpgroup
     }
-    mbar_init(bar_acc, 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc<TMEM_COLS>(smem_u32(&s_tmem));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = s_tmem;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (elect_one()) {
       tma_prefetch_desc(&tmDz);
       tma_prefetch_desc(&tmX);
@@ -117,74 +111,90 @@ wgrad_gemm_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constan
         if (++stage == num_stages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      const uint32_t idesc_full = umma_idesc_bf16(128, p.bn, 1, 1);
-      const uint32_t lcode_a = umma_layout_code(p.kc_a * 2);
-      const uint32_t lcode_b = umma_layout_code(p.kc_b * 2);
-      const uint32_t row_a = p.kc_a * 2, row_b = p.kc_b * 2;
-      // MN-major canonical layout: LBO = byte distance between channel boxes, SBO = 8 pixel rows.
-      // When the cout tile is narrower than 128 rows the extra rows alias box 0 (LBO 0): they only
-      // produce accumulator rows that the epilogue never reads.
-      const uint32_t lbo_a = (p.ma * p.kc_a >= 128) ? a_box_bytes : 0u;
-      const uint32_t lbo_b = b_box_bytes;
-      int stage = 0;
-      uint32_t phase = 0;
+  } else if (warp < 8) {
+    const int g = warp >> 2;                     // cout rows [64 g, 64 g + 64) of the tile
+    const int rows = p.ma * p.kc_a;              // cout rows of this tile's boxes (128, or the whole slice when narrower)
+    const bool active = 64 * g < rows;
+    const uint32_t lcode_a = gmma_layout_code(p.kc_a * 2);
+    const uint32_t lcode_b = gmma_layout_code(p.kc_b * 2);
+    const uint32_t row_a = p.kc_a * 2, row_b = p.kc_b * 2;
+    // MN-major canonical layout: LBO = byte distance between channel boxes, SBO = 8 pixel rows.  When the cout tile is narrower than
+    // 64 rows the extra rows alias box 0 (LBO 0): they only produce accumulator rows that are never stored.
+    const uint32_t lbo_a = rows >= 64 ? a_box_bytes : 0u;
+    const uint32_t a_off = static_cast<uint32_t>(64 * g / p.kc_a) * a_box_bytes;
+    int stage = 0, prev = -1;
+    uint32_t phase = 0;
+    if (!active) {  // no rows of this tile in this warpgroup: hand the slots back, nothing else
       for (int b = 0; b < nblk; ++b) {
         mbar_wait(bar_full + 8 * stage, phase);
-        tc_fence_after();
-        const uint32_t sa = smem_base + stage * stage_bytes;
-        for (int ti = 0; ti < ntap; ++ti) {
-          const uint32_t sb = sa + a_bytes + ti * b_tap_bytes;
-          const int ks = p.taps[tap0 + ti].ks;
-          const uint32_t idesc = ks > 0 ? umma_idesc_bf16(128, 16 * ks, 1, 1) : idesc_full;
-#pragma unroll
-          for (int k = 0; k < kWgPix / 16; ++k) {
-            const uint64_t da = umma_smem_desc(sa + k * 16 * row_a, lbo_a, 8 * row_a, lcode_a);
-            const uint64_t db = umma_smem_desc(sb + k * 16 * row_b, lbo_b, 8 * row_b, lcode_b);
-            umma_f16(tmem_base + ti * p.bn, da, db, idesc, (b | k) != 0 ? 1u : 0u);
-          }
-        }
-        umma_commit(bar_empty + 8 * stage);
+        mbar_arrive_if(bar_empty + 8 * prev, prev >= 0 && (threadIdx.x & 127) == 0);
+        prev = stage;
         if (++stage == num_stages) { stage = 0; phase ^= 1u; }
       }
-      umma_commit(bar_acc);
+      mbar_arrive_if(bar_empty + 8 * prev, prev >= 0 && (threadIdx.x & 127) == 0);
+      return;
     }
-  } else {
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const int co = cout_tile * 128 + row;
-    const bool row_ok = (row < p.ma * p.kc_a) && (co < p.cout);
-    if (nblk > 0) {
-      mbar_wait(bar_acc, 0);
-      tc_fence_after();
+    float acc[TPC][BN / 2];
+#pragma unroll
+    for (int ti = 0; ti < TPC; ++ti)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[ti][i] = 0.f;
+#pragma unroll
+    for (int ti = 0; ti < TPC; ++ti) wgmma_fence_operand(acc[ti]);  // opaque zeros: not rematerialised between the wgmma of a stage
+    for (int b = 0; b < nblk; ++b) {
+      mbar_wait(bar_full + 8 * stage, phase);
+      const uint32_t sa = smem_base + stage * stage_bytes;
+      wgmma_fence();
+      // every tap slot of the stage, also those of a short last tap group: their products land in accumulators that are never stored
+#pragma unroll
+      for (int ti = 0; ti < TPC; ++ti) {
+        const uint32_t sb = sa + a_bytes + ti * b_tap_bytes;
+#pragma unroll
+        for (int k = 0; k < kWgPix / 16; ++k)
+          Wgmma<BN>::template mma<1, 1>(acc[ti], gmma_desc(sa + a_off + k * 16 * row_a, lbo_a, 8 * row_a, lcode_a),
+                                        gmma_desc(sb + k * 16 * row_b, b_box_bytes, 8 * row_b, lcode_b), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous block's MMAs have completed: hand its slot back to the producer
+      mbar_arrive_if(bar_empty + 8 * prev, prev >= 0 && (threadIdx.x & 127) == 0);
+      prev = stage;
+      if (++stage == num_stages) { stage = 0; phase ^= 1u; }
     }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int ti = 0; ti < TPC; ++ti) wgmma_fence_operand(acc[ti]);
+    mbar_arrive_if(bar_empty + 8 * prev, prev >= 0 && (threadIdx.x & 127) == 0);
+
+    // accumulator fragment -> split-K workspace: thread rows r and r + 8, columns 8 i + 2 (lane % 4) + {0, 1}
+    const int r = 64 * g + 16 * (warp & 3) + (lane >> 2);
+    const int cpair = 2 * (lane & 3);
     float* wsb = p.ws + (long long)split * p.cout * p.num_taps * p.cin;
-    for (int ti = 0; ti < ntap; ++ti) {
-      float* dst = wsb + ((long long)co * p.num_taps + tap0 + ti) * p.cin + cin_tile * p.bn;
-      const int ks = p.taps[tap0 + ti].ks, shift = p.taps[tap0 + ti].kb;
-      for (int c = 0; c < p.bn; c += 16) {
-        uint32_t r[16];
-        const int src = ks > 0 ? c - shift : c;  // accumulator column of output column c (sparse taps: only [shift, shift + 16 ks) exist)
-        if (nblk > 0 && (ks == 0 || (src >= 0 && src < 16 * ks))) {
-          tmem_ld_32x16(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + ti * p.bn + src, r);
-          tmem_ld_wait();
-        } else {
 #pragma unroll
-          for (int i = 0; i < 16; ++i) r[i] = 0u;
-        }
-        if (row_ok) {
+    for (int hr = 0; hr < 2; ++hr) {
+      const int row = r + 8 * hr;
+      const int co = cout_tile * 128 + row;
+      if (row >= rows || co >= p.cout) continue;
 #pragma unroll
-          for (int i = 0; i < 16; i += 4)
-            *reinterpret_cast<uint4*>(dst + c + i) = make_uint4(r[i], r[i + 1], r[i + 2], r[i + 3]);
+      for (int ti = 0; ti < TPC; ++ti) {
+        if (ti >= ntap) continue;
+        float* dst = wsb + ((long long)co * p.num_taps + tap0 + ti) * p.cin + cin_tile * BN + cpair;
+        const int ks = p.taps[tap0 + ti].ks, shift = p.taps[tap0 + ti].kb;
+        if (ks == 0) {
+#pragma unroll
+          for (int i = 0; i < BN / 8; ++i)
+            *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(acc[ti][4 * i + 2 * hr], acc[ti][4 * i + 2 * hr + 1]);
+        } else {  // sparse tap: accumulator columns [0, 16 ks) belong at input channels [shift, shift + 16 ks)
+#pragma unroll
+          for (int i = 0; i < BN / 8; ++i)
+            if (8 * i < shift || 8 * i >= shift + 16 * ks) *reinterpret_cast<float2*>(dst + 8 * i) = make_float2(0.f, 0.f);
+#pragma unroll
+          for (int i = 0; i < BN / 8; ++i)
+            if (8 * i < 16 * ks && shift + 8 * i < BN)
+              *reinterpret_cast<float2*>(dst + shift + 8 * i) = make_float2(acc[ti][4 * i + 2 * hr], acc[ti][4 * i + 2 * hr + 1]);
         }
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<TMEM_COLS>(tmem_base);
 }
 
 // Sum the split-K partials and scatter into the reference's OIHW fp32 gradient layout

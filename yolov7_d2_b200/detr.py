@@ -1,16 +1,16 @@
-"""DETR transformer layers on the B200 kernels (forward path; SURVEY.md par.8a row T1).
+"""DETR transformer layers on the H100 kernels (forward path; SURVEY.md par.8a row T1).
 
 Reference: yolov7/modeling/backbone/detr_backbone.py -- `TransformerEncoderLayer` :128-187 (forward_post :157-170), `TransformerDecoderLayer`
 :190-279 (forward_post :221-242); both wrap torch's nn.MultiheadAttention (:140, :200-202).  The classes below keep the reference's
 constructor arguments, parameter names / shapes (`self_attn.in_proj_weight` [3E,E], `linear1.weight`, `norm1.weight` ...) and the seq-first
 `[L, B, E]` fp32 interface, and run
 
-    x (+pos) -> in_proj GEMMs (bias epilogue, q|k|v packed in one [B, L, 3E] buffer) -> yb200_attention_fwd (tcgen05, streaming softmax)
+    x (+pos) -> in_proj GEMMs (bias epilogue, q|k|v packed in one [B, L, 3E] buffer) -> yb200_attention_fwd (wgmma, streaming softmax)
       -> out_proj GEMM (+bias +residual epilogue) -> LayerNorm -> linear1 GEMM (+bias +ReLU epilogue) -> linear2 GEMM (+bias +residual) -> LayerNorm
 
 Internally tokens are batch-first bf16 `[B, 1, L, E]` views (yb200_act).  Forward and backward: with gradients enabled the layers run as one autograd node each
 (`_EncoderLayerFn` / `_DecoderLayerFn`: attention backward, data / weight gradients and LayerNorm backward on the same kernels), validated on
-hardware against the reference layer's autograd (tests/test_detr_gpu.py, round 2: 6 passed); YB200_DETR_TRAINING=0 forces the inference path.
+hardware against the reference layer's autograd (tests/test_detr_gpu.py); YB200_DETR_TRAINING=0 forces the inference path.
 Dropout (p = 0.1 in the reference: on the attention probabilities inside nn.MultiheadAttention and nn.Dropout on the residual branches / in the FFN) is
 active in training mode: the masks are a counter-based hash of (seed, element index) evaluated inside the kernels (yb200_attention_*_dropout,
 yb200_dropout), regenerated in the backward from the same seeds; seeds come from torch's CPU generator.  Same distribution as torch's Philox masks, not
@@ -286,7 +286,7 @@ class _LayerBase(nn.Module):
 
 class _EncoderLayerFn(torch.autograd.Function):
     """forward_post (detr_backbone.py:157-170) with everything the backward needs kept in bf16; backward = the chain
-    LayerNorm2 <- linear2 (+ReLU mask, fused) <- linear1 <- LayerNorm1 <- out_proj <- attention core <- in_proj on the B200 kernels"""
+    LayerNorm2 <- linear2 (+ReLU mask, fused) <- linear1 <- LayerNorm1 <- out_proj <- attention core <- in_proj on the H100 kernels"""
 
     NAMES = ("self_attn.in_proj_weight", "self_attn.in_proj_bias", "self_attn.out_proj.weight", "self_attn.out_proj.bias", "linear1.weight", "linear1.bias",
              "linear2.weight", "linear2.bias", "norm1.weight", "norm1.bias", "norm2.weight", "norm2.bias")
@@ -661,7 +661,7 @@ class Transformer(nn.Module):
                  normalize_before=False, return_intermediate_dec=False, device="cuda"):
         super().__init__()
         if normalize_before:
-            raise capi.Yb200Error("normalize_before=True (pre-norm) is not implemented by the B200 DETR layers")
+            raise capi.Yb200Error("normalize_before=True (pre-norm) is not implemented by the DETR layers of this package")
         enc = TransformerEncoderLayer(d_model, nhead, dim_feedforward, dropout, activation, normalize_before, device)
         self.encoder = TransformerEncoder(enc, num_encoder_layers, None)
         dec = TransformerDecoderLayer(d_model, nhead, dim_feedforward, dropout, activation, normalize_before, device)

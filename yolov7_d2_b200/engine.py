@@ -1,4 +1,4 @@
-"""Static execution plan of the YOLOX hot path on one B200: every tensor of the forward and backward pass is
+"""Static execution plan of the YOLOX hot path on one H100: every tensor of the forward and backward pass is
 allocated once (NHWC bf16 activations, concat buffers addressed through channel-slice views, fp32 flat parameter /
 gradient buffers) and a step is a fixed sequence of C-ABI kernel launches -- capturable in a CUDA graph.
 
@@ -726,8 +726,8 @@ class YoloxEngine:
         of its output?  That launch's epilogue then also performs the reduction pass of the head's BatchNorm backward
         (yb200_conv2d_dgrad_bnbwd), and the head only needs the apply pass.  Not fused: heads with an upsampled copy (their gradient has a
         second, 2x2-pooled source), heads whose gradient is finished by a non-convolution (SPP), gradient tensors of >= 256 channels and
-        more than two heads per launch.  Opt-in (YB200_BN_FUSE=1): measured on B200 (profiles/r2_bn_fusion_ab.md) the statistics cost the
-        epilogue-bound data-gradient kernels more (+3.4 ms per step) than the removed reduction pass saves (-2.4 ms), until z is staged by TMA."""
+        more than two heads per launch.  Opt-in (YB200_BN_FUSE=1): the statistics add dependent z loads and column sums to the data-gradient
+        epilogue, which already bounds those kernels, in exchange for the removed reduction pass."""
         self._bn_fuse = {}
         self._bn_fuse_idx = {}  # key -> (index of the writing op, [indices of the producing ops])
         op_index = {id(op): i for i, op in enumerate(self.ops)}

@@ -1,4 +1,4 @@
-"""Drop-in surface: the reference's registry / module contracts for the YOLOX path, backed by the B200 engine.
+"""Drop-in surface: the reference's registry / module contracts for the YOLOX path, backed by the H100 engine.
 
 Mirrors (same names, constructor arguments, attributes, state_dict keys and return types):
   * `@META_ARCH_REGISTRY.register() class YOLOX(nn.Module)`            yolov7/modeling/meta_arch/yolox.py:35-252
@@ -246,7 +246,7 @@ class CSPDarknet(Backbone, _Part):
     def __init__(self, dep_mul, wid_mul, out_features=("dark3", "dark4", "dark5"), depthwise=False, act="silu"):
         Backbone.__init__(self)
         if depthwise:
-            raise capi.Yb200Error("depthwise CSPDarknet is not implemented by the B200 path")
+            raise capi.Yb200Error("depthwise CSPDarknet is not implemented by this path")
         if act != "silu":
             raise AttributeError("Unsupported act type: {}".format(act))
         assert out_features, "please provide output features of Darknet"
@@ -285,7 +285,7 @@ class YOLOPAFPN(_Part):
     def __init__(self, depth=1.0, width=1.0, in_features=("dark3", "dark4", "dark5"), in_channels=[256, 512, 1024], depthwise=False, act="silu"):
         super().__init__()
         if depthwise:
-            raise capi.Yb200Error("depthwise YOLOPAFPN is not implemented by the B200 path")
+            raise capi.Yb200Error("depthwise YOLOPAFPN is not implemented by this path")
         self.in_features, self.in_channels = in_features, in_channels
         self._init_storage(80, width, depth)
 
@@ -309,7 +309,7 @@ class YOLOXHead(_Part):
     def __init__(self, num_classes, width=1.0, strides=[8, 16, 32], in_channels=[256, 512, 1024], act="silu", depthwise=False):
         super().__init__()
         if depthwise:
-            raise capi.Yb200Error("depthwise YOLOXHead is not implemented by the B200 path")
+            raise capi.Yb200Error("depthwise YOLOXHead is not implemented by this path")
         self.n_anchors, self.num_classes = 1, num_classes
         self.decode_in_inference = True
         self.use_l1 = False
@@ -428,7 +428,7 @@ class YOLOX(nn.Module):
         super().__init__()
         self.device = torch.device(cfg.MODEL.DEVICE)
         if self.device.type != "cuda":
-            raise capi.Yb200Error("the B200 YOLOX path needs MODEL.DEVICE = cuda")
+            raise capi.Yb200Error("the YOLOX path of this package needs MODEL.DEVICE = cuda")
         self.conf_threshold = cfg.MODEL.YOLO.CONF_THRESHOLD
         self.nms_threshold = cfg.MODEL.YOLO.NMS_THRESHOLD
         self.nms_type = cfg.MODEL.NMS_TYPE
@@ -578,10 +578,9 @@ class YOLOX(nn.Module):
                 for k, im in enumerate(imgs):  # separately allocated pinned images: one asynchronous DMA each, no host-side gather
                     images_dst[k].copy_(im, non_blocking=True)
             else:
-                # what a detectron2 dataloader hands over: a list of separately allocated pageable tensors.  Measured on the B200 box (2 x Xeon 8562Y+,
-                # profiles/r2_ab_runs.md): one asynchronous copy per image straight from pageable memory (the driver stages it) gives the best
-                # end-to-end rate; gathering into a pinned staging buffer costs less host time with a thread pool but not with torch.stack.
-                mode = os.environ.get("YB200_GATHER", "direct")  # direct | threads | stack (A/B knob, profiles/r2_ab_runs.md)
+                # what a detectron2 dataloader hands over: a list of separately allocated pageable tensors: by default one asynchronous copy per
+                # image straight from pageable memory (the driver stages it); a pinned staging buffer can be filled by a thread pool or torch.stack.
+                mode = os.environ.get("YB200_GATHER", "direct")  # direct | threads | stack (A/B knob)
                 if mode == "direct":  # one cudaMemcpyAsync per pageable image: the driver stages each through its own pinned buffers
                     for k, im in enumerate(imgs):
                         images_dst[k].copy_(im, non_blocking=True)

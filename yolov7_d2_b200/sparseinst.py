@@ -1,4 +1,4 @@
-"""SparseInst IAM decoder on the B200 kernels (forward path; SURVEY.md par.8a row S1).
+"""SparseInst IAM decoder on the H100 kernels (forward path; SURVEY.md par.8a row S1).
 
 Reference: yolov7/modeling/transcoders/decoder_sparseinst.py -- `InstanceBranch` :27-81, `MaskBranch` :84-104, `BaseIAMDecoder` :107-169.
 `BaseIAMDecoder(cfg)` below keeps the reference's constructor (the same `cfg.MODEL.SPARSE_INST.*` keys), parameter names / shapes
@@ -6,9 +6,9 @@ Reference: yolov7/modeling/transcoders/decoder_sparseinst.py -- `InstanceBranch`
 `mask_branch.mask_convs.*`, `mask_branch.projection.*`) and `forward(features NCHW fp32) -> {"pred_logits", "pred_masks", "pred_scores"[, "pred_iam"]}`.
 
 Kernel sequence (NHWC bf16 inside):
-  coordinates + features -> [B,H,W,Cpad]  |  4x conv3x3+bias+ReLU (tcgen05 implicit GEMM, `EPI_BF16_BIAS_RELU`) per branch
+  coordinates + features -> [B,H,W,Cpad]  |  4x conv3x3+bias+ReLU (wgmma implicit GEMM, `EPI_BF16_BIAS_RELU`) per branch
   iam = conv3x3+bias -> sigmoid -> per image:  raw = iam_prob^T features  (the pixel-contraction GEMM of the weight-gradient kernel: MN-major
-  UMMA descriptors straight on the NHWC tiles), normaliser = column sums, inst = raw / max(norm, 1e-6)
+  wgmma descriptors straight on the NHWC tiles), normaliser = column sums, inst = raw / max(norm, 1e-6)
   heads: three small GEMMs with fp32 output (`yb200_conv1x1_bias_f32`)  |  mask projection 1x1
   pred_masks = per-image 1x1 convolution of the mask features with pred_kernel[b] as weights, fp32 NCHW written by the GEMM epilogue
 The final bilinear x2 up-sampling (decoder_sparseinst.py:148-153) is `yb200_upsample_bilinear2x_f32` (other scale factors: F.interpolate).
@@ -117,7 +117,7 @@ class BaseIAMDecoder(nn.Module):
         return out
 
     def _aggregate(self, f, prob):
-        """inst[b] = prob[b]^T f[b] / clamp(sum prob[b], 1e-6)   (:70-76): the pixel contraction is the weight-gradient GEMM (MN-major UMMA
+        """inst[b] = prob[b]^T f[b] / clamp(sum prob[b], 1e-6)   (:70-76): the pixel contraction is the weight-gradient GEMM (MN-major wgmma
         descriptors on the NHWC tiles), per image; returns bf16 [B, 1, C_prob, dim]"""
         L, sp = self.L, capi.stream_ptr()
         b, dev, npad = f.shape[0], f.device, prob.shape[-1]

@@ -8,7 +8,7 @@ The shipped config is not runnable upstream: `build_convnext_backbone` returns s
       -> YOLOPAFPN(depth 0.33, width 0.75)   (in_channels = [256, 512, 1024] * 0.75 = [192, 384, 768])
       -> YOLOXHead(num_classes, width 0.75)  (hidden 192), SimOTA + IoU / BCE losses
 
-Two plans share the work: `ConvNeXtEngine` (csrc/convnext.cu kernels + the tcgen05 GEMM) and the neck + head range of a width-0.75
+Two plans share the work: `ConvNeXtEngine` (csrc/convnext.cu kernels + the wgmma GEMM) and the neck + head range of a width-0.75
 `YoloxEngine` (whose own CSPDarknet range never runs).  The object mirrors the YoloxEngine interface that modeling.YOLOX, bench.py and
 optim.py use (params / grads / buffers under the reference's `backbone.` / `neck.` / `head.` names, train_step, eval_forward, ...), with
 TWO flat parameter buffers (`flat_buffers()`): one optimizer launch and one all-reduce each.

@@ -79,22 +79,6 @@ int yb200_conv1x1_bias_f32(const yb200_act* x, const void* w_fwd, const float* b
  * input's shape, dz the output's.  addend may be NULL.                                                   */
 int yb200_conv2d_dgrad(const yb200_act* dz, const void* w_dgrad, const yb200_act* dx, const yb200_act* addend,
                        int ksize, int stride, void* stream);
-/* The same data gradient, whose epilogue ALSO performs the reduction pass of BatchNorm+SiLU backward for the layer(s) that
- * produced the activation whose gradient dx is (autograd of wrappers.py:76-80): for every segment, channels
- * [dx_c_begin, dx_c_begin + z.c) of dx are the final gradient of a = SiLU(z*scale + shift); the kernel accumulates
- * sum_du[c] += sum da*SiLU'(u), sum_duz[c] += sum da*SiLU'(u)*z  (fp64, c relative to the segment) while da is still in
- * registers, reading z (fp16, dx's pixel grid) once.  Feed the sums to yb200_bn_silu_bwd_apply.  dx must be the LAST
- * contribution to that gradient (addend = the earlier ones); gradient tensors of >= 256 channels are not supported.      */
-typedef struct yb200_bnbwd_seg {
-  yb200_act z;          /* fp16 pre-BatchNorm output of the producer (n, h, w as dx) */
-  int32_t dx_c_begin;   /* first channel of dx covered by this segment (multiple of 32) */
-  const float* scale;   /* per channel of the segment */
-  const float* shift;
-  double* sum_du;
-  double* sum_duz;
-} yb200_bnbwd_seg;
-int yb200_conv2d_dgrad_bnbwd(const yb200_act* dz, const void* w_dgrad, const yb200_act* dx, const yb200_act* addend,
-                             int ksize, int stride, int num_segments, const yb200_bnbwd_seg* segments, void* stream);
 
 /* grad_oihw (+)= d loss / d weight, fp32 [cout][cin_real][k][k] -- autograd of the convolution w.r.t. its weight.
  * workspace: at least yb200_conv2d_wgrad_workspace() bytes.                                              */
@@ -144,20 +128,12 @@ int yb200_bn_silu_bwd(const yb200_act* z, const yb200_act* da, const yb200_act* 
                       const float* scale, const float* shift, const float* save_mean, const float* save_invstd,
                       double* acc_dgamma, double* acc_dbeta, const yb200_act* dz, float* dgamma, float* dbeta,
                       int accumulate, void* stream);
-/* Second half of the same backward when the reduction already happened in the epilogue of yb200_conv2d_dgrad_bnbwd:
- * sum_duz / sum_du hold S2 = sum du*z and S1 = sum du (fp64 [c]; zeroed on exit).  dgamma = invstd*(S2 - mean*S1),
- * dbeta = S1, dz = scale*du - (scale*invstd*dgamma/M)*(z - mean) - scale*dbeta/M.                                      */
-int yb200_bn_silu_bwd_apply(const yb200_act* z, const yb200_act* da, const float* scale, const float* shift,
-                            const float* save_mean, const float* save_invstd, double* sum_duz, double* sum_du,
-                            const yb200_act* dz, float* dgamma, float* dbeta, int accumulate, void* stream);
 
-/* yb200_bn_silu_bwd / _apply with dgamma == dbeta == NULL leave their sums in the fp64 accumulators; this call converts the accumulators of a
+/* yb200_bn_silu_bwd with dgamma == dbeta == NULL leaves its sums in the fp64 accumulators; this call converts the accumulators of a
  * run of c channels (several layers) in one launch: grad_base[gamma_off[i]] (+)= dgamma_i, grad_base[beta_off[i]] (+)= dbeta_i, accumulators
- * zeroed.  raw_sums (may be NULL): per channel, 1 where the accumulators hold S2 / S1 of yb200_conv2d_dgrad_bnbwd (then save_mean / save_invstd
- * are read).  Replaces the tail of torch's batch_norm backward for every BaseConv of a plan (wrappers.py:60-80).                        */
+ * zeroed.  Replaces the tail of torch's batch_norm backward for every BaseConv of a plan (wrappers.py:60-80).                        */
 int yb200_bn_param_grads(double* acc_dgamma, double* acc_dbeta, int c, const int32_t* gamma_off, const int32_t* beta_off,
-                         float* grad_base, const float* save_mean, const float* save_invstd, const uint8_t* raw_sums,
-                         int accumulate, void* stream);
+                         float* grad_base, int accumulate, void* stream);
 
 /* ---- SPP / concat helpers ------------------------------------------------------------------------ */
 /* nn.MaxPool2d(k, 1, k//2) for k = 5, 9, 13 written into three channel slices (SPPBottleneck, wrappers.py:150-160).

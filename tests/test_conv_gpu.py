@@ -199,105 +199,3 @@ def test_conv_bn_silu_eval_fused(cuda, shape, with_res):
     if with_res:
         ref = ref.to(torch.bfloat16).float() + res.float()
     _close(out, ref, 2.0 ** -7, "fused out")
-
-
-# (N, H, W, Cin (= channels of dx), Cout (= channels of dz), k, stride, segment split of the dx channels)
-BNB_SHAPES = [
-    (8, 16, 16, 64, 32, 1, 1, (32, 32)),    # concat gradient: two producers (CSP conv3 reading [m-chain | conv2])
-    (8, 16, 16, 32, 32, 3, 1, (32,)),
-    (4, 40, 40, 64, 128, 3, 2, (64,)),      # stride 2: four parity launches accumulate into the same sums
-    (8, 20, 20, 128, 128, 3, 1, (128,)),
-    (3, 24, 36, 64, 64, 3, 1, (64,)),       # ragged tiles: masked rows must not count
-    (2, 80, 80, 128, 80, 1, 1, (128,)),     # prediction conv (cls, 80 channels of dz)
-    (8, 32, 32, 128, 64, 1, 1, (32, 64)),   # partial coverage: channels [96, 128) belong to no segment
-]
-
-
-@pytest.mark.parametrize("shape", BNB_SHAPES, ids=lambda s: "x".join(map(str, s[:7])))
-def test_conv_dgrad_fused_bn_backward_stats(cuda, shape):
-    """yb200_conv2d_dgrad_bnbwd: same dx as yb200_conv2d_dgrad, plus S1 = sum du and S2 = sum du*z per channel with
-    du = dx * SiLU'(z*scale + shift) -- the reduction pass of BatchNorm+SiLU backward (autograd of wrappers.py:76-80) on the stored
-    (bf16-rounded) gradient.  Reference: torch fp64 on the kernel's own dx."""
-    from yolov7_d2_b200 import capi
-
-    n, h, w, cin, cout, k, s, split = shape
-    L = capi.lib()
-    g = torch.Generator().manual_seed(21)
-    wt = (torch.randn(cout, cin, k, k, generator=g) / (cin * k * k) ** 0.5).to(torch.bfloat16).float().to(cuda)
-    _, wd = _pack(capi, wt, cout, cin)
-    dz = torch.randn(n, h // s, w // s, cout, generator=g).to(cuda).to(torch.bfloat16)
-    add = torch.randn(n, h, w, cin, generator=g).to(cuda).to(torch.bfloat16)
-    dx = torch.full((n, h, w, cin), float("nan"), dtype=torch.bfloat16, device=cuda)
-    dx_ref = torch.full_like(dx, float("nan"))
-    dza, dxa, dxra, adda = capi.act(dz), capi.act(dx), capi.act(dx_ref), capi.act(add)
-    capi.check(L.yb200_conv2d_dgrad(ctypes.byref(dza), capi.ptr(wd), ctypes.byref(dxra), ctypes.byref(adda), k, s, capi.stream_ptr()), "dgrad")
-    segs = (capi.BnBwdSeg * len(split))()
-    keep, begin = [], 0
-    for i, c in enumerate(split):
-        pitch = c + 32 * i  # the second producer's z lives in a wider (merged) tensor at a channel offset
-        zt = (torch.randn(n, h, w, pitch, generator=g) * 1.5).to(cuda).to(torch.float16)
-        scale = (torch.rand(c, generator=g) + 0.5).to(cuda)
-        shift = (torch.randn(c, generator=g) * 0.3).to(cuda)
-        s1 = torch.zeros(c, dtype=torch.float64, device=cuda)
-        s2 = torch.zeros(c, dtype=torch.float64, device=cuda)
-        segs[i].z = capi.act(zt, 32 * i, c)
-        segs[i].dx_c_begin = begin
-        segs[i].scale, segs[i].shift, segs[i].sum_du, segs[i].sum_duz = scale.data_ptr(), shift.data_ptr(), s1.data_ptr(), s2.data_ptr()
-        keep.append((zt, scale, shift, s1, s2, begin, c, 32 * i))
-        begin += c
-    capi.check(L.yb200_conv2d_dgrad_bnbwd(ctypes.byref(dza), capi.ptr(wd), ctypes.byref(dxa), ctypes.byref(adda), k, s, len(split), segs,
-                                          capi.stream_ptr()), "dgrad_bnbwd")
-    torch.cuda.synchronize()
-    assert torch.equal(dx, dx_ref), "the fused launch must produce the same gradient as the plain data-gradient kernel"
-    for zt, scale, shift, s1, s2, b0, c, zoff in keep:
-        z = zt[..., zoff:zoff + c].double()
-        da = dx[..., b0:b0 + c].double()
-        u = z * scale.double() + shift.double()
-        sg = torch.sigmoid(u)
-        du = da * sg * (1 + u * (1 - sg))
-        r1, r2 = du.sum((0, 1, 2)), (du * z).sum((0, 1, 2))
-        n1, n2 = du.abs().sum((0, 1, 2)), (du * z).abs().sum((0, 1, 2))
-        assert ((s1 - r1).abs() <= 2e-4 * n1 + 1e-6).all(), ((s1 - r1).abs() / n1).max().item()
-        assert ((s2 - r2).abs() <= 2e-4 * n2 + 1e-6).all(), ((s2 - r2).abs() / n2).max().item()
-
-
-def test_bn_silu_bwd_apply_equals_two_pass(cuda):
-    """yb200_bn_silu_bwd_apply on raw sums (S2, S1) == yb200_bn_silu_bwd (reduce + apply) on the same tensors"""
-    from yolov7_d2_b200 import capi
-
-    L = capi.lib()
-    g = torch.Generator().manual_seed(33)
-    n, h, w, c = 4, 24, 24, 64
-    z = (torch.randn(n, h, w, c, generator=g) * 1.3 + 0.2).to(cuda).to(torch.float16)
-    da = torch.randn(n, h, w, c, generator=g).to(cuda).to(torch.bfloat16)
-    gamma = (torch.rand(c, generator=g) + 0.5).to(cuda)
-    zf = z.float()
-    mean = zf.mean((0, 1, 2))
-    invstd = 1.0 / torch.sqrt(zf.var((0, 1, 2), unbiased=False) + 1e-3)
-    scale = gamma * invstd
-    shift = 0.1 - mean * scale
-    outs = []
-    for fused in (False, True):
-        a1 = torch.zeros(c, dtype=torch.float64, device=cuda)
-        a2 = torch.zeros(c, dtype=torch.float64, device=cuda)
-        dzt = torch.zeros(n, h, w, c, dtype=torch.bfloat16, device=cuda)
-        dg, db = torch.zeros(c, device=cuda), torch.zeros(c, device=cuda)
-        za, daa, dza = capi.act(z), capi.act(da), capi.act(dzt)
-        if fused:
-            u = zf * scale + shift
-            sg = torch.sigmoid(u)
-            du = (da.float() * sg * (1 + u * (1 - sg))).double()
-            a2.copy_(du.sum((0, 1, 2)))            # S1
-            a1.copy_((du * zf.double()).sum((0, 1, 2)))  # S2
-            capi.check(L.yb200_bn_silu_bwd_apply(ctypes.byref(za), ctypes.byref(daa), capi.ptr(scale), capi.ptr(shift), capi.ptr(mean), capi.ptr(invstd),
-                                                 capi.ptr(a1), capi.ptr(a2), ctypes.byref(dza), capi.ptr(dg), capi.ptr(db), 0, capi.stream_ptr()), "apply")
-        else:
-            capi.check(L.yb200_bn_silu_bwd(ctypes.byref(za), ctypes.byref(daa), None, None, capi.ptr(scale), capi.ptr(shift), capi.ptr(mean),
-                                           capi.ptr(invstd), capi.ptr(a1), capi.ptr(a2), ctypes.byref(dza), capi.ptr(dg), capi.ptr(db), 0,
-                                           capi.stream_ptr()), "bn_silu_bwd")
-        torch.cuda.synchronize()
-        assert float(a1.abs().sum()) == 0 and float(a2.abs().sum()) == 0, "accumulators must be zero on exit"
-        outs.append((dzt.float(), dg, db))
-    torch.testing.assert_close(outs[1][1], outs[0][1], rtol=2e-4, atol=1e-4)
-    torch.testing.assert_close(outs[1][2], outs[0][2], rtol=2e-4, atol=1e-4)
-    assert (outs[1][0] - outs[0][0]).abs().max() <= 2.0 ** -7 * outs[0][0].abs().max()

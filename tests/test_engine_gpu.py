@@ -191,33 +191,6 @@ def test_eval_forward_matches_oracle(step):
     assert e_eng.mean() <= 1.5 * e_emu.mean() + 1e-5
 
 
-def test_fused_bn_backward_statistics_equal_the_two_pass_path(step, cuda, monkeypatch):
-    """YB200_BN_FUSE=1 (BatchNorm-backward statistics from the data-gradient epilogue where the plan allows) vs the default two-pass kernels:
-    same step, same gradients up to 16-bit storage noise"""
-    from yolov7_d2_b200.engine import YoloxEngine
-
-    sd0 = step["sd0"]
-    monkeypatch.setenv("YB200_BN_FUSE", "1")
-    eng = YoloxEngine(step["eng"].n, step["eng"].h, step["eng"].w, device=cuda)
-    assert sum(hd.fused_stats for op in eng.ops if hasattr(op, "heads") for hd in op.heads) >= 40, "the plan fuses most BatchNorm layers"
-    monkeypatch.setenv("YB200_BN_FUSE", "0")
-    ref = YoloxEngine(eng.n, eng.h, eng.w, device=cuda)
-    assert not any(hd.fused_stats for op in ref.ops if hasattr(op, "heads") for hd in op.heads)
-    grads = []
-    for e in (eng, ref):
-        e.load_state_dict(sd0)
-        e.images_u8.copy_(step["images"].to(cuda))
-        e.labels.copy_(step["labels"].to(cuda))
-        e.train_step()
-        torch.cuda.synchronize()
-        grads.append({n: e.grads[n].clone() for n in e.param_names})
-    assert torch.allclose(eng.losses, ref.losses, rtol=1e-6)
-    for n in eng.param_names:
-        a, b = grads[0][n].flatten().double(), grads[1][n].flatten().double()
-        cos = float((a @ b) / (a.norm() * b.norm() + 1e-30))
-        assert cos >= 0.999 and abs(float(a.norm() / (b.norm() + 1e-30)) - 1) <= 0.02, (n, cos)
-
-
 def test_pixel_grouped_stem_equals_plain_stem(step, cuda, monkeypatch):
     """YB200_STEM_GROUP4 (default on): the stem convolution and its weight gradient run on [N, H, W/4, 64] views (128-byte TMA rows) with an
     expanded weight matrix; same pre-BatchNorm output, statistics and parameter gradient as the plain 16-channel formulation"""

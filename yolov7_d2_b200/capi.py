@@ -41,19 +41,6 @@ class Act(ctypes.Structure):
     ]
 
 
-class BnBwdSeg(ctypes.Structure):
-    """mirror of `yb200_bnbwd_seg` (include/yb200.h)"""
-
-    _fields_ = [
-        ("z", Act),
-        ("dx_c_begin", ctypes.c_int32),
-        ("scale", c_void_p),
-        ("shift", c_void_p),
-        ("sum_du", c_void_p),
-        ("sum_duz", c_void_p),
-    ]
-
-
 class PackDesc(ctypes.Structure):
     """mirror of `yb200_pack_desc` (include/yb200.h)"""
 

@@ -4,7 +4,6 @@
 #include "wgrad_gemm.cuh"
 
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
 
 namespace yb {
@@ -20,9 +19,9 @@ static int launch_conv_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
   // memory allows after the epilogue staging tiles
   const int phases = p.num_phases == 4 ? 4 : 1;
   const int m_tiles = grid.x * phases, n_tiles = grid.y;  // work items of one column tile (pixel tiles x output-parity phases)
-  const int occ = conv_min_ctas(BN, BK, p.num_bnseg > 0 ? 2 : 0);
+  const int occ = conv_min_ctas(BN, BK);
   // fp32 rows with channel stride 1 and an odd pitch ([B, A, 85]): chunks go through a per-warp transpose scratch behind the ring
-  const bool xpose = p.epi_mode == EPI_F32_BIAS && p.out_sc == 1 && p.num_bnseg == 0;
+  const bool xpose = p.epi_mode == EPI_F32_BIAS && p.out_sc == 1;
   const int fixed = ConvEpiCfg<BN>::kStageBytes + (xpose ? kXposeBytes : 0);
   const int budget = (occ == 1 ? 212 : 104) * 1024 - 1024 - fixed;
   int slots_kb = budget / Cfg::kStageBytes;  // k-blocks that fit in the ring
@@ -40,26 +39,20 @@ static int launch_conv_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
   static PerDevice<int> max_set_p_dev(0);
   int& max_set_p = max_set_p_dev.cur();
   if (smem > max_set_p) {
-    YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_persistent_kernel<BN, BK, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_persistent_kernel<BN, BK, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_persistent_kernel<BN, BK, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_persistent_kernel<BN, BK, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     max_set_p = smem;
   }
   int groups = (occ * sm_count()) / n_tiles;
   if (groups < 1) groups = 1;
   if (groups > m_tiles) groups = m_tiles;
   if (phases == 4 && groups > 1 && groups % 2 == 0) --groups;  // odd stride through the work items: every CTA cycles through all four phases (1 / 2 / 2 / 4 taps)
-  if (p.num_bnseg > 0) {  // data gradient with fused BatchNorm-backward statistics
-    YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_persistent_kernel<BN, BK, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    launch_k(conv_gemm_persistent_kernel<BN, BK, 2>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, p, pst, kbs, n_tiles, m_tiles);
-    YB_CHECK_CUDA(cudaGetLastError());
-    return 0;
-  }
   ConvGemmParams pp = p;
   pp.xpose = xpose ? 1 : 0;
   if (ext)
-    launch_k(conv_gemm_persistent_kernel<BN, BK, 1>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, pp, pst, kbs, n_tiles, m_tiles);
+    launch_k(conv_gemm_persistent_kernel<BN, BK, true>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, pp, pst, kbs, n_tiles, m_tiles);
   else
-    launch_k(conv_gemm_persistent_kernel<BN, BK, 0>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, pp, pst, kbs, n_tiles, m_tiles);
+    launch_k(conv_gemm_persistent_kernel<BN, BK, false>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, pp, pst, kbs, n_tiles, m_tiles);
   YB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -121,7 +114,7 @@ static void set_out_view(ConvGemmParams& p, const yb200_act& o) {
   p.out_sh = 1LL * o.c_pitch * o.w;
   p.out_sn = 1LL * o.c_pitch * o.w * o.h;
   p.out_sc = 1;
-  p.out_mh = 1; p.out_ph = 0; p.out_mw = 1; p.out_pw = 0;
+  p.out_mh = 1; p.out_mw = 1;
 }
 
 static void set_tiles(ConvGemmParams& p, int n, int h, int w) {
@@ -296,14 +289,9 @@ static int conv_fwd_common(const yb200_act* x, const void* w_fwd, int cout, int 
     // right neighbour only its first.  The side taps therefore load / multiply `cpp` channels instead of group * cpp: their activation box starts
     // at the needed pixel (the rest of the box lies beyond the channel extent: TMA zero fill, no L2 traffic) and the weight box at the matching
     // columns.  The products beyond the first cpp channels are zero either way (zero-filled activations on the left, zero weights of the
-    // expanded matrix on the right); YB200_STEM_SPARSE=0 keeps the dense taps for A/B runs.
-    static int sparse = -1;
-    if (sparse < 0) {
-      const char* e = getenv("YB200_STEM_SPARSE");
-      sparse = (e && e[0] == '0') ? 0 : 1;
-    }
+    // expanded matrix on the right).
     const int cpp = x->c / group;
-    for (int t = 0; t < p.num_taps && sparse; ++t) {
+    for (int t = 0; t < p.num_taps; ++t) {
       ConvTap& tp = p.taps[t];
       if (tp.dw == -1) { tp.c0 += (group - 1) * cpp; tp.kb += (group - 1) * cpp; }
     }
@@ -600,8 +588,7 @@ extern "C" int yb200_conv1x1_bias_f32_split(const yb200_act* x, int lo_delta, in
 // data gradient
 // ------------------------------------------------------------------------------------------------
 static int dgrad_impl(const yb200_act* dz, const void* w_dgrad, const yb200_act* dx, const yb200_act* addend, int ksize, int stride,
-                      const yb200_act* gelu_u, double* colsum, void* stream, int act_mode = EPI_BF16_GELU_BWD, int num_seg = 0,
-                      const yb200_bnbwd_seg* segs = nullptr) {
+                      const yb200_act* gelu_u, double* colsum, void* stream, int act_mode = EPI_BF16_GELU_BWD) {
   int rc;
   if ((rc = check_act(dz, "conv2d_dgrad dz"))) return rc;
   if ((rc = check_act(dx, "conv2d_dgrad dx"))) return rc;
@@ -637,31 +624,7 @@ static int dgrad_impl(const yb200_act* dz, const void* w_dgrad, const yb200_act*
     p.add_sh = 1LL * addend->c_pitch * addend->w;
     p.add_sn = 1LL * addend->c_pitch * addend->w * addend->h;
   }
-  if (num_seg > 0) {
-    YB_REQUIRE(num_seg <= 2 && segs != nullptr && gelu_u == nullptr, YB200_ERR_INVALID, "conv2d_dgrad_bnbwd: 1 or 2 segments");
-    YB_REQUIRE(bn <= 128, YB200_ERR_UNSUPPORTED, "conv2d_dgrad_bnbwd: gradient tensors of %d channels use a 256-wide column tile (not supported)", cin);
-    p.num_bnseg = num_seg;
-    for (int i = 0; i < num_seg; ++i) {
-      const yb200_bnbwd_seg& sgm = segs[i];
-      const yb200_act& z = sgm.z;
-      YB_REQUIRE(z.ptr && sgm.scale && sgm.shift && sgm.sum_du && sgm.sum_duz, YB200_ERR_INVALID, "conv2d_dgrad_bnbwd: null pointer in segment %d", i);
-      YB_REQUIRE(z.n == dx->n && z.h == dx->h && z.w == dx->w && z.c % 32 == 0 && sgm.dx_c_begin % 32 == 0 && sgm.dx_c_begin >= 0 &&
-                     sgm.dx_c_begin + z.c <= dx->c && z.c_off % 8 == 0 && z.c_pitch % 8 == 0,
-                 YB200_ERR_INVALID, "conv2d_dgrad_bnbwd: segment %d (z %dx%dx%dx%d at dx channel %d) does not fit dx %dx%dx%dx%d", i, z.n, z.h, z.w, z.c,
-                 sgm.dx_c_begin, dx->n, dx->h, dx->w, dx->c);
-      BnBwdSeg& d = p.bnseg[i];
-      d.col_begin = sgm.dx_c_begin;
-      d.col_end = sgm.dx_c_begin + z.c;
-      d.z = static_cast<const __half*>(z.ptr) + z.c_off;
-      d.z_sw = z.c_pitch;
-      d.z_sh = 1LL * z.c_pitch * z.w;
-      d.z_sn = 1LL * z.c_pitch * z.w * z.h;
-      d.scale = sgm.scale; d.shift = sgm.shift; d.sum_du = sgm.sum_du; d.sum_duz = sgm.sum_duz;
-    }
-    YB_REQUIRE(num_seg < 2 || p.bnseg[0].col_end <= p.bnseg[1].col_begin || p.bnseg[1].col_end <= p.bnseg[0].col_begin, YB200_ERR_INVALID,
-               "conv2d_dgrad_bnbwd: overlapping segments");
-  }
-  set_tiles(p, dz->n, dz->h, dz->w);  // pixel grid = dz grid (for stride 2: one output-parity class at a time)
+  set_tiles(p, dz->n, dz->h, dz->w);  // pixel grid = dz grid (for stride 2: each work item is one output-parity class of a tile)
   const int tw = 1 << p.log_tw, th = 1 << p.log_th, tn = 128 >> (p.log_tw + p.log_th);
   CUtensorMap tmA, tmB;
   if ((rc = make_act_map(&tmA, *dz, false, bk, tw, th, tn))) return rc;
@@ -696,43 +659,22 @@ static int dgrad_impl(const yb200_act* dz, const void* w_dgrad, const yb200_act*
     return nt;
   };
   p.out_mh = 2; p.out_mw = 2;
-  static int one_launch = -1;  // YB200_DGRAD_PHASES=4 restores one launch per output-parity class (A/B runs)
-  if (one_launch < 0) {
-    const char* e = getenv("YB200_DGRAD_PHASES");
-    one_launch = (e && e[0] == '4') ? 0 : 1;
-  }
-  if (one_launch) {
-    // all four phases in ONE persistent launch: the phases of a pixel tile run back to back on neighbouring CTAs and share its dz tile in L2
-    int nt = 0;
-    for (int ph = 0; ph < 2; ++ph)
-      for (int pw = 0; pw < 2; ++pw) {
-        p.phase_tap[ph * 2 + pw] = nt;
-        nt += phase_taps(ph, pw, p.taps + nt);
-      }
-    p.phase_tap[4] = nt;
-    p.num_taps = nt;
-    p.num_phases = 4;
-    return launch_conv(bn, bk, tmA, tmB, p, grid, st);
-  }
+  // all four phases in ONE persistent launch: the phases of a pixel tile run back to back on neighbouring CTAs and share its dz tile in L2
+  int nt = 0;
   for (int ph = 0; ph < 2; ++ph)
     for (int pw = 0; pw < 2; ++pw) {
-      const int nt = phase_taps(ph, pw, p.taps);
-      p.num_taps = nt;
-      p.out_ph = ph; p.out_pw = pw;
-      if ((rc = launch_conv(bn, bk, tmA, tmB, p, grid, st))) return rc;
+      p.phase_tap[ph * 2 + pw] = nt;
+      nt += phase_taps(ph, pw, p.taps + nt);
     }
-  return 0;
+  p.phase_tap[4] = nt;
+  p.num_taps = nt;
+  p.num_phases = 4;
+  return launch_conv(bn, bk, tmA, tmB, p, grid, st);
 }
 
 extern "C" int yb200_conv2d_dgrad(const yb200_act* dz, const void* w_dgrad, const yb200_act* dx, const yb200_act* addend,
                                   int ksize, int stride, void* stream) {
   return dgrad_impl(dz, w_dgrad, dx, addend, ksize, stride, nullptr, nullptr, stream);
-}
-
-extern "C" int yb200_conv2d_dgrad_bnbwd(const yb200_act* dz, const void* w_dgrad, const yb200_act* dx, const yb200_act* addend, int ksize, int stride,
-                                        int num_segments, const yb200_bnbwd_seg* segments, void* stream) {
-  YB_REQUIRE(num_segments >= 1, YB200_ERR_INVALID, "conv2d_dgrad_bnbwd: no segments (use yb200_conv2d_dgrad)");
-  return dgrad_impl(dz, w_dgrad, dx, addend, ksize, stride, nullptr, nullptr, stream, EPI_BF16, num_segments, segments);
 }
 
 extern "C" int yb200_linear_dgrad_gelu(const yb200_act* dh_src, const void* w_dgrad, const yb200_act* u, const yb200_act* du, double* bias_grad_sum,
@@ -797,12 +739,7 @@ int plan_wgrad(const yb200_act* x, const yb200_act* dz, int ksize, int stride, W
     YB_REQUIRE(ksize == 3 && stride == 1 && x->c % group == 0 && cpp % 16 == 0 && x->c_off == 0 && x->c == x->c_pitch && p.cin_tiles == 1 && p.nb == 1,
                YB200_ERR_UNSUPPORTED, "conv2d_wgrad_grouped: needs a 3x3 stride-1 convolution on a whole [.., %d x 16k]-channel grouped tensor of <= 64 channels (got c=%d pitch=%d group=%d)",
                group, x->c, x->c_pitch, group);
-    static int sparse = -1;
-    if (sparse < 0) {
-      const char* e = getenv("YB200_STEM_SPARSE");
-      sparse = (e && e[0] == '0') ? 0 : 1;
-    }
-    for (int t = 0; t < p.num_taps && sparse; ++t) {
+    for (int t = 0; t < p.num_taps; ++t) {
       ConvTap& tp = p.taps[t];
       tp.kb = 0;
       if (tp.dw == -1) { tp.c0 += (group - 1) * cpp; tp.kb = (group - 1) * cpp; tp.ks = cpp / 16; }
@@ -821,16 +758,8 @@ int plan_wgrad(const yb200_act* x, const yb200_act* dz, int ksize, int stride, W
   const int occ_regs = p.tpc * p.bn <= 96 ? 2 : 1;  // CTAs per SM the accumulator registers allow (wgrad_gemm_kernel launch bounds)
   const int stage = kWgPix * 2 * (p.kc_a * p.ma + p.kc_b * p.nb * p.tpc);
   p.stages = kWgStages;
-  if (std::min(occ_regs, (220 * 1024) / (stage * kWgStages + 1024)) <= 1) {  // one CTA per SM anyway: deepen the ring (YB200_WGRAD_STAGES caps it, A/B)
-    static int cap = -1;
-    if (cap < 0) {
-      const char* e = getenv("YB200_WGRAD_STAGES");
-      cap = e ? atoi(e) : kWgMaxStages;
-      if (cap < kWgStages) cap = kWgStages;
-      if (cap > kWgMaxStages) cap = kWgMaxStages;
-    }
-    p.stages = std::max(kWgStages, std::min(cap, (220 * 1024 - 1024) / stage));
-  }
+  if (std::min(occ_regs, (220 * 1024) / (stage * kWgStages + 1024)) <= 1)  // one CTA per SM anyway: deepen the ring
+    p.stages = std::max(kWgStages, std::min(kWgMaxStages, (220 * 1024 - 1024) / stage));
   pl->smem = stage * p.stages + 1024;
   // Split the pixel range so that ONE wave of CTAs covers the machine (every CTA pays pipeline fill and a full accumulator
   // write-back, so extra waves are pure overhead); occupancy is bounded by registers and shared memory.
@@ -863,7 +792,7 @@ static int launch_wgrad_inst(const CUtensorMap& tmDz, const CUtensorMap& tmX, co
     YB_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BN, TPC>, cudaFuncAttributeMaxDynamicSharedMemorySize, pl.smem));
     max_set = pl.smem;
   }
-  launch_k_opt(use_pdl_wgrad(), wgrad_gemm_kernel<BN, TPC>, grid, kWgThreads, pl.smem, st, tmDz, tmX, pl.p);
+  launch_k_opt(false, wgrad_gemm_kernel<BN, TPC>, grid, kWgThreads, pl.smem, st, tmDz, tmX, pl.p);
   YB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
@@ -907,7 +836,7 @@ static int wgrad_impl(const yb200_act* x, const yb200_act* dz, int ksize, int st
   if (rc) return rc;
   const long long total = 1LL * pl.p.cout * pl.p.num_taps * pl.p.cin;
   const int blocks = static_cast<int>(std::min<long long>((total + 31) / 32, 16 * sm_count()));
-  launch_k_opt(use_pdl_wgrad(), wgrad_reduce_kernel, blocks, 256, 0, st, pl.p.ws, grad_oihw, pl.splits, pl.p.cout, pl.p.num_taps, pl.p.cin, cin_real, accumulate);
+  launch_k_opt(false, wgrad_reduce_kernel, blocks, 256, 0, st, pl.p.ws, grad_oihw, pl.splits, pl.p.cout, pl.p.num_taps, pl.p.cin, cin_real, accumulate);
   YB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -68,32 +68,17 @@ struct ConvTap {
   int ks;  // > 0: only the first ks 16-wide K steps of each k-block of this tap carry non-zero operands (persistent kernel: the rest is skipped)
 };
 
-// Fused BatchNorm-backward statistics (kernel variant 2, data-gradient launches): the epilogue that produces the FINAL gradient da of an
-// activation a = SiLU(BN(z)) also reads z and accumulates  S1 = sum du,  S2 = sum du * z  with du = da * SiLU'(z*scale + shift)  per channel
-// -- the reduction pass of BatchNorm backward (dbeta = S1, dgamma = invstd * (S2 - mean * S1)) without a second trip of da and z through HBM.
-// Up to two segments: the gradient tensor may be a concat buffer whose channel ranges come from different BatchNorm layers.
-struct BnBwdSeg {
-  int col_begin, col_end;      // columns (channels of the gradient tensor being written) covered by this segment; multiples of 32
-  const __half* z;             // the producer's pre-BN output, pointing at (pixel 0, channel col_begin)
-  long long z_sn, z_sh, z_sw;  // element strides of z over (image, row, column); z has the geometry of the gradient tensor
-  const float* scale;          // BatchNorm scale / shift of the producer, indexed by (column - col_begin)
-  const float* shift;
-  double* sum_du;              // S1 accumulator, indexed by (column - col_begin)
-  double* sum_duz;             // S2 accumulator
-};
-
 struct ConvGemmParams {
-  int num_bnseg;
-  BnBwdSeg bnseg[2];
   int tiles_w, tiles_h, tiles_n;
   int log_tw, log_th;          // tile = (1<<log_tw) x (1<<log_th) x (128 >> (log_tw+log_th)) pixels
   int num_taps, cin_blocks;    // K loop = num_taps * cin_blocks blocks of BLOCK_K
   int n_valid, h_valid, w_valid;  // pixel-grid extents (tile-space); pixels outside are neither stored nor counted
   int cout;                    // valid output channels (columns >= cout are dropped)
   int epi_mode;
-  // output element (n, y, x, c) lives at out[n*out_sn + (y*out_mh+out_ph)*out_sh + (x*out_mw+out_pw)*out_sw + c*out_sc]
+  // output element (n, y, x, c) lives at out[n*out_sn + (y*out_mh+ph)*out_sh + (x*out_mw+pw)*out_sw + c*out_sc]; (ph, pw) is the
+  // output-parity phase of the work item when num_phases == 4, else (0, 0)
   long long out_sn, out_sh, out_sw;
-  int out_sc, out_mh, out_ph, out_mw, out_pw;
+  int out_sc, out_mh, out_mw;
   void* out;
   const __nv_bfloat16* addend;  // optional, bf16, same (n,y,x) -> offset mapping with its own strides, channel stride 1
   long long add_sn, add_sh, add_sw;
@@ -125,7 +110,7 @@ __device__ __forceinline__ void conv_decode_work(const ConvGemmParams& p, int wi
     oph = ph >> 1;
     opw = ph & 1;
   } else {
-    m = wi; tap0 = 0; ntaps = p.num_taps; oph = p.out_ph; opw = p.out_pw;
+    m = wi; tap0 = 0; ntaps = p.num_taps; oph = opw = 0;
   }
 }
 
@@ -177,38 +162,6 @@ __device__ __forceinline__ void stage_col_params(const ConvGemmParams& p, int co
   }
 }
 
-__device__ __forceinline__ int bnseg_of(const ConvGemmParams& p, int col) {
-  if (p.num_bnseg > 0 && col >= p.bnseg[0].col_begin && col < p.bnseg[0].col_end) return 0;
-  if (p.num_bnseg > 1 && col >= p.bnseg[1].col_begin && col < p.bnseg[1].col_end) return 1;
-  return -1;
-}
-template <int BLOCK_N>
-__device__ __forceinline__ void stage_col_params_bnseg(const ConvGemmParams& p, int col0, float (*s_col)[BLOCK_N]) {
-  for (int i = threadIdx.x; i < BLOCK_N; i += blockDim.x) {
-    const int s = bnseg_of(p, col0 + i);
-    s_col[0][i] = s >= 0 ? p.bnseg[s].scale[col0 + i - p.bnseg[s].col_begin] : 1.f;
-    s_col[1][i] = s >= 0 ? p.bnseg[s].shift[col0 + i - p.bnseg[s].col_begin] : 0.f;
-  }
-}
-__device__ __forceinline__ float silu_grad_f(float u, float d) {  // d * d/du [u * sigmoid(u)], sigmoid on MUFU.TANH as elementwise.cu
-  float t;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * u));
-  const float sg = fmaf(t, 0.5f, 0.5f);
-  return (d * sg) * fmaf(u, 1.f - sg, 1.f);
-}
-// fp16 z chunk of one pixel row (CH channels) for the fused BatchNorm-backward statistics
-template <int CH>
-__device__ __forceinline__ void load_z_chunk(const __half* zrow, bool valid, uint4 (&dst)[CH / 8]) {
-#pragma unroll
-  for (int k = 0; k < CH / 8; ++k) {
-    dst[k] = make_uint4(0u, 0u, 0u, 0u);
-    if (valid) {
-      const void* ptr = zrow + 8 * k;
-      asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(dst[k].x), "=r"(dst[k].y), "=r"(dst[k].z), "=r"(dst[k].w) : "l"(ptr));
-    }
-  }
-}
-
 // EXT = false: the YOLOX training / inference modes only (EPI_BF16 .. EPI_BF16_BN_SILU); EXT = true adds the ConvNeXt / transformer
 // modes.  Two instantiations per kernel keep the hot YOLOX kernels free of the extra modes' registers and code.
 // fp32 rows with a pitch that is not a multiple of 16 bytes (the [B, A, 85] prediction tensor): a lane-per-pixel store touches 32 different
@@ -219,8 +172,7 @@ constexpr int kXposeBytes = 8 * kXposeWarpFloats * 4;       // eight epilogue wa
 template <int CH, bool EXT = true>
 __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, float (&v)[CH], bool valid, long long pix_off, long long add_off,
                                                     int cbase, int lane, float* part_sum, float* part_sq, bool accumulate,
-                                                    const float* col_scale, const float* col_shift,
-                                                    const uint4* zq = nullptr, float* xp = nullptr) {
+                                                    const float* col_scale, const float* col_shift, float* xp = nullptr) {
   if (p.epi_mode == EPI_F32_BIAS) {
     if (xp != nullptr) {
       long long* s_off = reinterpret_cast<long long*>(xp + 32 * 33);
@@ -343,7 +295,7 @@ __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, flo
   // round once (one packed conversion per two values; the kernels that carry this epilogue are bound by its instruction count on the narrow
   // layers, ncu: ~50 % issue-slot utilisation with 8 epilogue warps per CTA); statistics describe exactly the values that are stored
   const bool f16 = p.epi_mode == EPI_F16 || p.epi_mode == EPI_F16_STATS;
-  const bool need_vals = p.epi_mode == EPI_F16_STATS || zq != nullptr || (EXT && p.stat_sum != nullptr);
+  const bool need_vals = p.epi_mode == EPI_F16_STATS || (EXT && p.stat_sum != nullptr);
   if (f16) {
     uint32_t pk[CH / 2];
 #pragma unroll
@@ -381,36 +333,6 @@ __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, flo
         v[i + 1] = valid ? bf16_hi(pk[i >> 1]) : 0.f;
       }
     }
-  }
-  if (zq != nullptr) {
-    // fused BatchNorm-backward statistics on the values just stored (v = rounded da; 0 on masked rows): du -> v, du * z -> zf
-    float zf[CH];
-#pragma unroll
-    for (int k = 0; k < CH / 8; ++k) {
-      const uint32_t w4[4] = {zq[k].x, zq[k].y, zq[k].z, zq[k].w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        __half2 h;
-        *reinterpret_cast<uint32_t*>(&h) = w4[j];
-        const float2 f = __half22float2(h);
-        zf[8 * k + 2 * j] = f.x;
-        zf[8 * k + 2 * j + 1] = f.y;
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < CH; ++i) {
-      const float du = silu_grad_f(fmaf(zf[i], col_scale[i], col_shift[i]), v[i]);
-      v[i] = du;
-      zf[i] *= du;
-    }
-    float cs, cq;
-    if constexpr (CH == 32) { cs = warp_colsum32(v, lane); cq = warp_colsum32(zf, lane); }
-    else { cs = warp_colsum16(v, lane); cq = warp_colsum16(zf, lane); }
-    if (lane < CH) {
-      part_sum[lane] = accumulate ? part_sum[lane] + cs : cs;
-      part_sq[lane] = accumulate ? part_sq[lane] + cq : cq;
-    }
-    return;
   }
   if (p.epi_mode == EPI_F16_STATS) {
     float sq[CH];
@@ -455,20 +377,17 @@ struct ConvEpiCfg {
   static constexpr int kStageBytes = 2 * 64 * kPitch * 4;     // both warpgroups
 };
 
-__host__ __device__ constexpr int conv_min_ctas(int block_n, int block_k, int var) { return (block_n >= 128 || var == 2 || block_k == 16) ? 1 : 2; }
+__host__ __device__ constexpr int conv_min_ctas(int block_n, int block_k) { return (block_n >= 128 || block_k == 16) ? 1 : 2; }
 
-// VAR: 0 = YOLOX training / inference epilogues, 1 = + ConvNeXt / transformer epilogues (EXT), 2 = data gradient with fused
-// BatchNorm-backward statistics (BnBwdSeg; epi_mode EPI_BF16)
-template <int BLOCK_N, int BLOCK_K, int VAR>
+// EXT: false = YOLOX training / inference epilogues, true = + ConvNeXt / transformer epilogues
+template <int BLOCK_N, int BLOCK_K, bool EXT>
 // two CTAs per SM (96 registers per thread: five of their 18 warps share one 16 K-register SM sub-partition) where that fits without
-// spilling; one CTA per SM (168 registers) for BN 128, for VAR 2 (the z loads) and for BLOCK_K 16 (the deep k-block slots); conv_min_ctas
-__global__ void __launch_bounds__(kConvThreadsP, conv_min_ctas(BLOCK_N, BLOCK_K, VAR))
+// spilling; one CTA per SM (168 registers) for BN 128 and for BLOCK_K 16 (the deep k-block slots); conv_min_ctas
+__global__ void __launch_bounds__(kConvThreadsP, conv_min_ctas(BLOCK_N, BLOCK_K))
 conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                             const __grid_constant__ ConvGemmParams p, int num_stages, int kb_per_slot, int n_tiles, int m_tiles) {
   using Cfg = ConvGemmCfg<BLOCK_N, BLOCK_K>;
   using Epi = ConvEpiCfg<BLOCK_N>;
-  constexpr bool EXT = VAR == 1;
-  constexpr bool BNB = VAR == 2;
   constexpr int CH = Epi::kChunk;
   extern __shared__ uint8_t smem_dyn[];
   __shared__ __align__(8) uint64_t s_bar[2 * kMaxStagesP];
@@ -498,8 +417,7 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
   }
   for (int i = threadIdx.x; i < 4 * 2 * BLOCK_N; i += blockDim.x) (&s_part[0][0][0])[i] = 0.f;
   pdl_sync();  // everything above touches only this CTA's shared memory: it overlaps the tail of the previous kernel
-  if constexpr (BNB) stage_col_params_bnseg<BLOCK_N>(p, col0, s_col);
-  else stage_col_params<BLOCK_N>(p, col0, s_col);
+  stage_col_params<BLOCK_N>(p, col0, s_col);
   __syncthreads();
 
   if (warp == 8) {
@@ -547,7 +465,7 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
     const int nl = mrow >> (log_tw + log_th);
     float* const stg = reinterpret_cast<float*>(smem_al + ring_bytes) + g * 64 * Epi::kPitch;
     float* xp = nullptr;
-    if (!BNB && p.xpose) xp = reinterpret_cast<float*>(smem_al + ring_bytes + Epi::kStageBytes) + warp * kXposeWarpFloats;
+    if (p.xpose) xp = reinterpret_cast<float*>(smem_al + ring_bytes + Epi::kStageBytes) + warp * kXposeWarpFloats;
     constexpr uint32_t lcode = gmma_layout_code(Cfg::kSwizzle);
     constexpr uint32_t sbo = 8 * Cfg::kSwizzle;  // 8 rows of one swizzle atom
     float acc[BLOCK_N / 2];
@@ -596,15 +514,6 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
                                 (long long)(x * p.out_mw + opw) * p.out_sw;
       const long long add_off = (long long)n * p.add_sn + (long long)(y * p.out_mh + oph) * p.add_sh +
                                 (long long)(x * p.out_mw + opw) * p.add_sw;
-      // fused BatchNorm-backward statistics: this pixel's row of z in each segment
-      const __half* zrow[2] = {nullptr, nullptr};
-      if constexpr (BNB) {
-#pragma unroll
-        for (int sg = 0; sg < 2; ++sg)
-          if (sg < p.num_bnseg)
-            zrow[sg] = p.bnseg[sg].z + (long long)n * p.bnseg[sg].z_sn + (long long)(y * p.out_mh + oph) * p.bnseg[sg].z_sh +
-                       (long long)(x * p.out_mw + opw) * p.bnseg[sg].z_sw - p.bnseg[sg].col_begin;
-      }
       float* const r0 = stg + (16 * wl + (lane >> 2)) * Epi::kPitch + 2 * (lane & 3);  // this thread's fragment rows in the staging tile
       float* const r1 = r0 + 8 * Epi::kPitch;
       const float* const row_src = stg + ((wl & 1) * 32 + lane) * Epi::kPitch + half * CH;
@@ -629,31 +538,14 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
             const float4 f = *reinterpret_cast<const float4*>(row_src + i);
             v[i] = f.x; v[i + 1] = f.y; v[i + 2] = f.z; v[i + 3] = f.w;
           }
-          uint4 zq[CH / 8];
-          int zseg = -1;
-          if constexpr (BNB) {
-            zseg = bnseg_of(p, col0 + c);  // warp-uniform: chunks never straddle a segment boundary
-            if (zseg >= 0) load_z_chunk<CH>(zrow[zseg] + col0 + c, valid, zq);
-          }
           conv_epilogue_chunk<CH, EXT>(p, v, valid, pix_off, add_off, col0 + c, lane, &s_part[q][0][c], &s_part[q][1][c], true, &s_col[0][c],
-                                       &s_col[1][c], (BNB && zseg >= 0) ? zq : nullptr, xp);
+                                       &s_col[1][c], xp);
         }
       }
     }
   }
 
   __syncthreads();
-  if constexpr (BNB) {
-    for (int e = threadIdx.x; e < BLOCK_N && col0 + e < p.cout; e += blockDim.x) {
-      const int sg = bnseg_of(p, col0 + e);
-      if (sg < 0) continue;
-      const float s1 = (s_part[0][0][e] + s_part[1][0][e]) + (s_part[2][0][e] + s_part[3][0][e]);
-      const float s2 = (s_part[0][1][e] + s_part[1][1][e]) + (s_part[2][1][e] + s_part[3][1][e]);
-      atomicAdd(p.bnseg[sg].sum_du + col0 + e - p.bnseg[sg].col_begin, static_cast<double>(s1));
-      atomicAdd(p.bnseg[sg].sum_duz + col0 + e - p.bnseg[sg].col_begin, static_cast<double>(s2));
-    }
-    return;
-  }
   if (EXT ? epi_has_stats(p.epi_mode, p.stat_sum) : p.epi_mode == EPI_F16_STATS) {
     for (int e = threadIdx.x; e < BLOCK_N && col0 + e < p.cout; e += blockDim.x) {  // BLOCK_N may exceed the thread count
       const float s1 = (s_part[0][0][e] + s_part[1][0][e]) + (s_part[2][0][e] + s_part[3][0][e]);

@@ -422,7 +422,7 @@ template <bool SIMPLE>
 __global__ void __launch_bounds__(kEwThreads, 3)
 bn_silu_bwd_apply_kernel(View z, DaSrc da, View dz, const float* __restrict__ scale, const float* __restrict__ shift,
                          const float* __restrict__ mean, const float* __restrict__ invstd, const double* __restrict__ dgamma_acc,
-                         const double* __restrict__ dbeta_acc, double inv_count, unsigned npix, int raw_sums) {
+                         const double* __restrict__ dbeta_acc, double inv_count, unsigned npix) {
   pdl_sync();
   const int c8 = threadIdx.x * 8;
   float s[8], t[8], A[8], B[8];
@@ -430,9 +430,7 @@ bn_silu_bwd_apply_kernel(View z, DaSrc da, View dz, const float* __restrict__ sc
   for (int k = 0; k < 8; ++k) {
     s[k] = scale[c8 + k]; t[k] = shift[c8 + k];
     const float is = invstd[c8 + k], mu = mean[c8 + k];
-    // raw_sums: the accumulators hold S2 = sum du*z and S1 = sum du (fused into the data-gradient epilogue): dgamma = invstd * (S2 - mean*S1)
-    const double dg = raw_sums ? static_cast<double>(is) * (dgamma_acc[c8 + k] - static_cast<double>(mu) * dbeta_acc[c8 + k]) : dgamma_acc[c8 + k];
-    const float mg = static_cast<float>(dg * inv_count);
+    const float mg = static_cast<float>(dgamma_acc[c8 + k] * inv_count);
     const float mb = static_cast<float>(dbeta_acc[c8 + k] * inv_count);
     A[k] = -s[k] * is * mg;
     B[k] = -s[k] * mb - A[k] * mu;
@@ -467,13 +465,11 @@ bn_silu_bwd_apply_kernel(View z, DaSrc da, View dz, const float* __restrict__ sc
 
 // parameter gradients out of the fp64 accumulators, then re-zero them
 __global__ void bn_param_grad_kernel(double* __restrict__ dgamma_acc, double* __restrict__ dbeta_acc, int c, float* __restrict__ dgamma,
-                                     float* __restrict__ dbeta, int accumulate, const float* __restrict__ mean, const float* __restrict__ invstd,
-                                     int raw_sums) {
+                                     float* __restrict__ dbeta, int accumulate) {
   pdl_sync();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= c) return;
-  const double dg = raw_sums ? static_cast<double>(invstd[i]) * (dgamma_acc[i] - static_cast<double>(mean[i]) * dbeta_acc[i]) : dgamma_acc[i];
-  const float g = static_cast<float>(dg), b = static_cast<float>(dbeta_acc[i]);
+  const float g = static_cast<float>(dgamma_acc[i]), b = static_cast<float>(dbeta_acc[i]);
   dgamma[i] = accumulate ? dgamma[i] + g : g;
   dbeta[i] = accumulate ? dbeta[i] + b : b;
   dgamma_acc[i] = 0.0;
@@ -768,9 +764,9 @@ extern "C" int yb200_bn_train_apply_silu(const yb200_act* z, const double* stat_
   return bn_apply_impl(z, nullptr, nullptr, residual, out, out_up2x, fin, stream);
 }
 
-static int bn_silu_bwd_impl(const yb200_act* z, const yb200_act* da, const yb200_act* da2, const yb200_act* da_up2x, const float* scale,
-                            const float* shift, const float* save_mean, const float* save_invstd, double* acc_dgamma, double* acc_dbeta,
-                            const yb200_act* dz, float* dgamma, float* dbeta, int accumulate, void* stream, int stats_ready) {
+extern "C" int yb200_bn_silu_bwd(const yb200_act* z, const yb200_act* da, const yb200_act* da2, const yb200_act* da_up2x, const float* scale,
+                                 const float* shift, const float* save_mean, const float* save_invstd, double* acc_dgamma, double* acc_dbeta,
+                                 const yb200_act* dz, float* dgamma, float* dbeta, int accumulate, void* stream) {
   int rc;
   if ((rc = check_view(z, "bn_silu_bwd z")) || (rc = check_view(da, "bn_silu_bwd da")) || (rc = check_view(dz, "bn_silu_bwd dz"))) return rc;
   if (da2 && (rc = check_view(da2, "bn_silu_bwd da2"))) return rc;
@@ -795,62 +791,43 @@ static int bn_silu_bwd_impl(const yb200_act* z, const yb200_act* da, const yb200
   // pixels per thread in the reduction pass: up to 32, fewer for small tensors so that >= ~6 blocks per SM exist
   int red_iters = static_cast<int>(npix / (static_cast<long long>(block.y) * 6 * sm_count()));
   red_iters = red_iters < 4 ? 4 : (red_iters > kBnRedIters ? kBnRedIters : red_iters);
-  const unsigned grid_r = static_cast<unsigned>((npix + block.y * red_iters - 1) / (block.y * red_iters));
   const bool red_shuffle = cv < 32 && (cv & (cv - 1)) == 0;
   const int red_rows = red_shuffle ? static_cast<int>(block.x * block.y) / 32 : static_cast<int>(block.y);
   const size_t red_smem = static_cast<size_t>(red_rows) * 2 * z->c * sizeof(float);
-  // tuning knob (tools/bench_bn.py): YB200_BN_RED = "U:MINB:ITERS" -- loads in flight per thread, resident blocks per SM, pixels per thread
-  static int red_u = -1, red_minb = 3, red_it = 0;  // default U = 2 loads in flight, 3 blocks / SM
-  if (red_u < 0) {
-    red_u = 2;
-    const char* e = getenv("YB200_BN_RED");
-    if (e) sscanf(e, "%d:%d:%d", &red_u, &red_minb, &red_it);
+  const unsigned grid_r = static_cast<unsigned>((npix + block.y * red_iters - 1) / (block.y * red_iters));
+  if (src.has_b || src.has_up) {  // fan-out / upsampled gradient sources: the general kernel
+    if (red_smem > 48 * 1024)
+      YB_CHECK_CUDA(cudaFuncSetAttribute(bn_silu_bwd_reduce_kernel<2, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(red_smem)));
+    launch_k(bn_silu_bwd_reduce_kernel<2, 3, false>, grid_r, block, red_smem, st, vz, src, scale, shift, save_mean, save_invstd, acc_dgamma, acc_dbeta,
+                                                                             static_cast<unsigned>(npix), red_iters, l2_order());
+  } else {
+    if (red_smem > 48 * 1024)
+      YB_CHECK_CUDA(cudaFuncSetAttribute(bn_silu_bwd_reduce_kernel<2, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(red_smem)));
+    launch_k(bn_silu_bwd_reduce_kernel<2, 3, true>, grid_r, block, red_smem, st, vz, src, scale, shift, save_mean, save_invstd, acc_dgamma, acc_dbeta,
+                                                                            static_cast<unsigned>(npix), red_iters, l2_order());
   }
-  if (red_it > 0) red_iters = red_it;
-  const unsigned grid_r2 = static_cast<unsigned>((npix + block.y * red_iters - 1) / (block.y * red_iters));
-  if (!stats_ready) {
-    if (src.has_b || src.has_up) {  // fan-out / upsampled gradient sources: the general kernel
-      if (red_smem > 48 * 1024)
-        YB_CHECK_CUDA(cudaFuncSetAttribute(bn_silu_bwd_reduce_kernel<2, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(red_smem)));
-      launch_k(bn_silu_bwd_reduce_kernel<2, 3, false>, grid_r2, block, red_smem, st, vz, src, scale, shift, save_mean, save_invstd, acc_dgamma, acc_dbeta,
-                                                                               static_cast<unsigned>(npix), red_iters, l2_order());
-    } else
-#define YB_RED(UU, MB)                                                                                                                     \
-  if (red_u == UU && red_minb == MB) {                                                                                                     \
-    if (red_smem > 48 * 1024)                                                                                                              \
-      YB_CHECK_CUDA(cudaFuncSetAttribute(bn_silu_bwd_reduce_kernel<UU, MB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(red_smem))); \
-    launch_k(bn_silu_bwd_reduce_kernel<UU, MB, true>, grid_r2, block, red_smem, st, vz, src, scale, shift, save_mean, save_invstd, acc_dgamma, acc_dbeta,   \
-                                                                        static_cast<unsigned>(npix), red_iters, l2_order());                \
-  } else
-    YB_RED(1, 3) YB_RED(2, 3) YB_RED(4, 3) YB_RED(1, 4) YB_RED(2, 4) YB_RED(4, 4) YB_RED(2, 2) YB_RED(4, 2) YB_RED(1, 6) YB_RED(2, 6)
-    return fail(YB200_ERR_INVALID, "YB200_BN_RED: no reduce variant U=%d MINB=%d", red_u, red_minb);
-#undef YB_RED
-    YB_CHECK_CUDA(cudaGetLastError());
-  }
+  YB_CHECK_CUDA(cudaGetLastError());
   const unsigned grid_a = static_cast<unsigned>((npix + block.y * kEwIters - 1) / (block.y * kEwIters));
   if (!src.has_b && !src.has_up)
     launch_k(bn_silu_bwd_apply_kernel<true>, grid_a, block, 0, st, vz, src, vdz, scale, shift, save_mean, save_invstd, acc_dgamma, acc_dbeta,
-                                                              1.0 / static_cast<double>(npix), static_cast<unsigned>(npix), stats_ready);
+                                                              1.0 / static_cast<double>(npix), static_cast<unsigned>(npix));
   else
     launch_k(bn_silu_bwd_apply_kernel<false>, grid_a, block, 0, st, vz, src, vdz, scale, shift, save_mean, save_invstd, acc_dgamma, acc_dbeta,
-                                                               1.0 / static_cast<double>(npix), static_cast<unsigned>(npix), stats_ready);
+                                                               1.0 / static_cast<double>(npix), static_cast<unsigned>(npix));
   YB_CHECK_CUDA(cudaGetLastError());
   if (dgamma == nullptr) return 0;  // deferred: yb200_bn_param_grads turns the accumulators of many layers into parameter gradients in one launch
-  launch_k(bn_param_grad_kernel, ceil_div(z->c, 128), 128, 0, st, acc_dgamma, acc_dbeta, z->c, dgamma, dbeta, accumulate, save_mean, save_invstd, stats_ready);
+  launch_k(bn_param_grad_kernel, ceil_div(z->c, 128), 128, 0, st, acc_dgamma, acc_dbeta, z->c, dgamma, dbeta, accumulate);
   YB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
 // the same for a run of layers: channel i of the run writes grad_base[gamma_off[i]] / grad_base[beta_off[i]]
 __global__ void bn_param_grads_table_kernel(double* __restrict__ dgamma_acc, double* __restrict__ dbeta_acc, int c, const int* __restrict__ gamma_off,
-                                            const int* __restrict__ beta_off, float* __restrict__ grad_base, int accumulate,
-                                            const float* __restrict__ mean, const float* __restrict__ invstd, const uint8_t* __restrict__ raw) {
+                                            const int* __restrict__ beta_off, float* __restrict__ grad_base, int accumulate) {
   pdl_sync();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= c) return;
-  const bool is_raw = raw != nullptr && raw[i] != 0;
-  const double dg = is_raw ? static_cast<double>(invstd[i]) * (dgamma_acc[i] - static_cast<double>(mean[i]) * dbeta_acc[i]) : dgamma_acc[i];
-  const float g = static_cast<float>(dg), b = static_cast<float>(dbeta_acc[i]);
+  const float g = static_cast<float>(dgamma_acc[i]), b = static_cast<float>(dbeta_acc[i]);
   float* pg = grad_base + gamma_off[i];
   float* pb = grad_base + beta_off[i];
   *pg = accumulate ? *pg + g : g;
@@ -860,25 +837,11 @@ __global__ void bn_param_grads_table_kernel(double* __restrict__ dgamma_acc, dou
 }
 
 extern "C" int yb200_bn_param_grads(double* acc_dgamma, double* acc_dbeta, int c, const int32_t* gamma_off, const int32_t* beta_off, float* grad_base,
-                                    const float* save_mean, const float* save_invstd, const uint8_t* raw_sums, int accumulate, void* stream) {
-  YB_REQUIRE(acc_dgamma && acc_dbeta && gamma_off && beta_off && grad_base && c > 0 && (!raw_sums || (save_mean && save_invstd)), YB200_ERR_INVALID,
-             "bn_param_grads: bad arguments");
-  launch_k(bn_param_grads_table_kernel, ceil_div(c, 128), 128, 0, as_stream(stream), acc_dgamma, acc_dbeta, c, gamma_off, beta_off, grad_base, accumulate,
-                                                                               save_mean, save_invstd, raw_sums);
+                                    int accumulate, void* stream) {
+  YB_REQUIRE(acc_dgamma && acc_dbeta && gamma_off && beta_off && grad_base && c > 0, YB200_ERR_INVALID, "bn_param_grads: bad arguments");
+  launch_k(bn_param_grads_table_kernel, ceil_div(c, 128), 128, 0, as_stream(stream), acc_dgamma, acc_dbeta, c, gamma_off, beta_off, grad_base, accumulate);
   YB_CHECK_CUDA(cudaGetLastError());
   return 0;
-}
-
-extern "C" int yb200_bn_silu_bwd(const yb200_act* z, const yb200_act* da, const yb200_act* da2, const yb200_act* da_up2x, const float* scale,
-                                 const float* shift, const float* save_mean, const float* save_invstd, double* acc_dgamma, double* acc_dbeta,
-                                 const yb200_act* dz, float* dgamma, float* dbeta, int accumulate, void* stream) {
-  return bn_silu_bwd_impl(z, da, da2, da_up2x, scale, shift, save_mean, save_invstd, acc_dgamma, acc_dbeta, dz, dgamma, dbeta, accumulate, stream, 0);
-}
-
-extern "C" int yb200_bn_silu_bwd_apply(const yb200_act* z, const yb200_act* da, const float* scale, const float* shift, const float* save_mean,
-                                       const float* save_invstd, double* sum_duz, double* sum_du, const yb200_act* dz, float* dgamma, float* dbeta,
-                                       int accumulate, void* stream) {
-  return bn_silu_bwd_impl(z, da, nullptr, nullptr, scale, shift, save_mean, save_invstd, sum_duz, sum_du, dz, dgamma, dbeta, accumulate, stream, 1);
 }
 
 extern "C" int yb200_spp_pool(const yb200_act* x, const yb200_act* o5, const yb200_act* o9, const yb200_act* o13, uint8_t* argmax, void* stream) {

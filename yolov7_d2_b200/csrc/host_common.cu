@@ -1,7 +1,5 @@
 #include "host_common.cuh"
 
-#include <stdlib.h>
-
 #include <mutex>
 
 namespace yb {
@@ -16,24 +14,6 @@ int fail(int code, const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
   return code;
-}
-
-bool use_pdl() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("YB200_PDL");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-bool use_pdl_wgrad() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("YB200_PDL_WGRAD");
-    v = (e && e[0] == '1') ? 1 : 0;  // default off: parked weight-gradient CTAs hold shared memory the main stream needs
-  }
-  return v == 1;
 }
 
 int current_device() {

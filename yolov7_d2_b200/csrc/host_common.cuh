@@ -56,10 +56,9 @@ void choose_tile(int n, int h, int w, int npix, int* log_tw, int* log_th);
 // Programmatic dependent launch: every kernel of the YOLOX path starts with pdl_sync() (griddepcontrol.wait, then launch_dependents) and is
 // launched through launch_k with the programmatic-stream-serialization attribute.  The next kernel of the stream (or of the captured graph) is
 // then scheduled while this one drains: its CTAs take the SM slots that free up and park at their own griddepcontrol.wait until this grid has
-// completed and flushed -- launch latency and block scheduling of ~540 launches per step leave the critical path.  YB200_PDL=0 launches plainly.
-bool use_pdl();
-bool use_pdl_wgrad();  // the weight-gradient kernels (side stream) launch plainly unless YB200_PDL_WGRAD=1: a parked CTA of theirs holds up to 160 KB of
-                       // shared memory that the main stream's kernels then cannot use
+// completed and flushed -- launch latency and block scheduling of ~540 launches per step leave the critical path.  The weight-gradient kernels
+// (side stream) launch plainly through launch_k_opt(false, ...): a parked CTA of theirs holds up to 160 KB of shared memory that the main
+// stream's kernels then cannot use.
 template <typename... K, typename... A>
 inline cudaError_t launch_k_opt(bool pdl, void (*kernel)(K...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
   cudaLaunchConfig_t cfg = {};
@@ -71,22 +70,12 @@ inline cudaError_t launch_k_opt(bool pdl, void (*kernel)(K...), dim3 grid, dim3 
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
-  cfg.numAttrs = (pdl && use_pdl()) ? 1 : 0;
+  cfg.numAttrs = pdl ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
 }
 template <typename... K, typename... A>
 inline cudaError_t launch_k(void (*kernel)(K...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = use_pdl() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
+  return launch_k_opt(true, kernel, grid, block, smem, st, std::forward<A>(args)...);
 }
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }

@@ -131,7 +131,6 @@ class YoloxEngine:
         self._build()
         self._alloc_params(share_params_of)
         self._alloc_runtime()
-        self._plan_bn_fusion()
 
     # ------------------------------------------------------------------ graph construction
     def _buf(self, name, h, w, c, dtype=torch.bfloat16):
@@ -304,7 +303,6 @@ class YoloxEngine:
                         base = (self.grads[hd.prefix + leaf].data_ptr() - self.flat_grad.data_ptr()) // 4
                         dst[hd.bn_off:hd.bn_off + hd.c] = torch.arange(base, base + hd.c, dtype=torch.int32)
         self.bn_goff, self.bn_boff = g_off.to(dev), b_off.to(dev)
-        self._bn_raw = None
         self.flat_nbt = share.flat_nbt if share is not None else torch.zeros(len(nbt), dtype=torch.int64, device=dev)
         for i, name in enumerate(nbt):
             self.buffers[name] = self.flat_nbt[i]
@@ -721,97 +719,6 @@ class YoloxEngine:
                                           p_dcls, p_dro, None, bias_acc, sp), what)
 
     # ------------------------------------------------------------------ backward
-    def _plan_bn_fusion(self):
-        """Static analysis of the backward pass: for every BatchNorm head, which data-gradient launch writes the FINAL value of the gradient
-        of its output?  That launch's epilogue then also performs the reduction pass of the head's BatchNorm backward
-        (yb200_conv2d_dgrad_bnbwd), and the head only needs the apply pass.  Not fused: heads with an upsampled copy (their gradient has a
-        second, 2x2-pooled source), heads whose gradient is finished by a non-convolution (SPP), gradient tensors of >= 256 channels and
-        more than two heads per launch.  Opt-in (YB200_BN_FUSE=1): the statistics add dependent z loads and column sums to the data-gradient
-        epilogue, which already bounds those kernels, in exchange for the removed reduction pass."""
-        self._bn_fuse = {}
-        self._bn_fuse_idx = {}  # key -> (index of the writing op, [indices of the producing ops])
-        op_index = {id(op): i for i, op in enumerate(self.ops)}
-        for op in self.ops:
-            if isinstance(op, ConvOp):
-                for hd in op.heads:
-                    hd.fused_stats = False
-        if self.strict or os.environ.get("YB200_BN_FUSE", "0") != "1":
-            return
-        writers = {}  # id(buffer) -> [(lo, hi, key)] in backward order
-        for op in reversed(self.ops):
-            if isinstance(op, PredOp):
-                for which, feat in (("cls", op.cls_feat), ("reg", op.reg_feat)):
-                    writers.setdefault(id(feat.buf), []).append((feat.off, feat.off + feat.c, ("pred", id(op), which)))
-            elif isinstance(op, SppOp):
-                v = op.views[0]
-                writers.setdefault(id(v.buf), []).append((v.off, v.off + v.c, ("spp", id(op), None)))
-            elif not op.first:
-                writers.setdefault(id(op.x.buf), []).append((op.x.off, op.x.off + op.x.c, ("conv", id(op), None)))
-        for op in self.ops:
-            if not isinstance(op, ConvOp):
-                continue
-            for hd in op.heads:
-                v = hd.out
-                if hd.up is not None or hd.c % 32 != 0 or v.off % 32 != 0:
-                    continue
-                ws = [w for w in writers.get(id(v.buf), []) if not (w[1] <= v.off or v.off + v.c <= w[0])]
-                if not ws:
-                    continue
-                lo, hi, key = ws[-1]
-                if key[0] == "spp" or not (lo <= v.off and v.off + v.c <= hi) or hi - lo >= 256 or (v.off - lo) % 32 != 0:
-                    continue
-                segs = self._bn_fuse.setdefault(key, [])
-                if len(segs) < 2:
-                    segs.append((hd, op, v.off - lo))
-                    hd.fused_stats = True
-                    self._bn_fuse_idx.setdefault(key, (op_index[key[1]], []))[1].append(op_index[id(op)])
-        raw = torch.zeros(self.nbn, dtype=torch.uint8)  # channels whose accumulators hold the raw sums S2 / S1 of the fused epilogue
-        for op in self.ops:
-            if isinstance(op, ConvOp):
-                for hd in op.heads:
-                    if hd.fused_stats:
-                        raw[hd.bn_off:hd.bn_off + hd.c] = 1
-        self._bn_raw = raw.to(self.dev) if bool(raw.any()) else None
-
-    def _range_fusable(self, op_range):
-        """a partial backward keeps the fused statistics when every fused launch has its writer and its producers on the same side of the
-        range boundaries (otherwise accumulators would be fed without being consumed, or consumed without being fed)"""
-        if op_range is None:
-            return True
-        lo, hi = op_range
-        inside = lambda i: lo <= i < hi
-        return all(all(inside(p) == inside(w) for p in prods) for w, prods in self._bn_fuse_idx.values())
-
-    def _bn_segments(self, key):
-        """ctypes array of yb200_bnbwd_seg for the data-gradient launch `key` (None when nothing is fused into it)"""
-        segs = self._bn_fuse.get(key) if getattr(self, "_fuse_active", True) else None
-        if not segs:
-            return None, 0
-        cached = getattr(self, "_bn_seg_cache", None)
-        if cached is None:
-            cached = self._bn_seg_cache = {}
-        if key not in cached:
-            nb, f8 = self.nbn, self.flat_stats
-            arr = (capi.BnBwdSeg * len(segs))()
-            for i, (hd, op, begin) in enumerate(segs):
-                arr[i].z = capi.act(op.z.buf.t, hd.c0, hd.c)
-                arr[i].dx_c_begin = begin
-                arr[i].scale = self.flat_scale.data_ptr() + 4 * hd.bn_off
-                arr[i].shift = self.flat_shift.data_ptr() + 4 * hd.bn_off
-                arr[i].sum_duz = f8.data_ptr() + 8 * (2 * nb + hd.bn_off)
-                arr[i].sum_du = f8.data_ptr() + 8 * (3 * nb + hd.bn_off)
-            cached[key] = arr
-        return cached[key], len(segs)
-
-    def _dgrad(self, dz_act, w_dgrad, dx_view, addend_act, ksize, stride, key, what):
-        L, sp = self.L, capi.stream_ptr()
-        segs, nseg = self._bn_segments(key)
-        if nseg:
-            capi.check(L.yb200_conv2d_dgrad_bnbwd(dz_act, capi.ptr(w_dgrad), dx_view.gact(), addend_act, ksize, stride, nseg, segs, sp), what)
-        else:
-            capi.check(L.yb200_conv2d_dgrad(dz_act, capi.ptr(w_dgrad), dx_view.gact(), addend_act, ksize, stride, sp), what)
-        return nseg
-
     def _grouped_views(self, op, dz=None):
         """the stem's input / output (or output gradient) seen as [N, H, W/4, 4C]: same memory, 4 pixels per row"""
         xb = op.x.buf
@@ -888,7 +795,7 @@ class YoloxEngine:
         """op_range = (lo, hi): backward of self.ops[lo:hi] only, from gradients the caller has already stored in the gradient buffers of
         the `seeded` views (standalone backbone / neck / head, modeling.py), or -- fresh=False -- continuing a backward pass that earlier
         calls ran over the later ranges (dist.GradientBuckets: the gradient bucket of a finished range is all-reduced while the next range
-        computes).  A range keeps the fused BatchNorm statistics only if no fused launch pairs an op inside it with one outside."""
+        computes)."""
         if self.strict:
             raise capi.Yb200Error("strict mode is a forward / loss verification mode: no backward (use the default engine for training)")
         L, sp = self.L, capi.stream_ptr()
@@ -900,7 +807,6 @@ class YoloxEngine:
                 b.written = []
         for v in seeded:
             v.buf.written.append((v.off, v.off + v.c))
-        self._fuse_active = self._range_fusable(op_range)
         lo_i, hi_i = op_range if op_range is not None else (0, len(self.ops))
         pending_res = {}  # id(view.buf), off -> gradient view of the residual sum
         for op in reversed(self.ops[lo_i:hi_i]):
@@ -915,7 +821,7 @@ class YoloxEngine:
                 for which, feat, dz, gdst, wd in (("cls", op.cls_feat, dcls, op.gc_dst, op.wc_dgrad), ("reg", op.reg_feat, dro, op.gr_dst, op.wr_dgrad)):
                     self._wgrad(feat.act(), ctypes.byref(dz), 1, 1, self.hc, gdst, acc, "pred")
                     add = self._grad_target(feat)
-                    self._dgrad(ctypes.byref(dz), wd, feat, add.gact() if add else None, 1, 1, ("pred", id(op), which), "pred dgrad")
+                    capi.check(L.yb200_conv2d_dgrad(ctypes.byref(dz), capi.ptr(wd), feat.gact(), add.gact() if add else None, 1, 1, sp), "pred dgrad")
                 self._count(7, "pred level %d: bias_grad, 2x(wgrad, reduce, dgrad)" % k, "pred_conv bwd", self.n * h * w * 2.0 * (4 * self.hc + self.nc + 16),
                             4.0 * self.n * h * w * self.hc * (self.nc + 5))
             elif isinstance(op, SppOp):
@@ -934,19 +840,12 @@ class YoloxEngine:
                     dzv = dzb.view(hd.c0, hd.c)
                     o = hd.bn_off
                     npx = op.z.buf.n * op.z.buf.h * op.z.buf.w
-                    if hd.fused_stats and self._fuse_active:  # the reduction pass ran in the epilogue of the data gradient that produced hd.out's gradient
-                        capi.check(L.yb200_bn_silu_bwd_apply(zv.act(), hd.out.gact(), pf(self.flat_scale, o), pf(self.flat_shift, o), pf(self.flat_mean, o),
-                                                             pf(self.flat_invstd, o), ctypes.c_void_p(f8.data_ptr() + 8 * (2 * nb + o)),
-                                                             ctypes.c_void_p(f8.data_ptr() + 8 * (3 * nb + o)), dzv.act(), None, None,
-                                                             acc, sp), "bn_silu_bwd_apply " + hd.prefix)
-                        self._count(1, "bn_bwd (apply; reduce fused upstream) %s c=%d px=%d" % (hd.prefix, hd.c, npx), "bn_silu_bwd", 6.0 * npx * hd.c)
-                    else:
-                        capi.check(L.yb200_bn_silu_bwd(zv.act(), hd.out.gact(), None, hd.up.gact() if hd.up else None, pf(self.flat_scale, o),
-                                                       pf(self.flat_shift, o), pf(self.flat_mean, o), pf(self.flat_invstd, o),
-                                                       ctypes.c_void_p(f8.data_ptr() + 8 * (2 * nb + o)), ctypes.c_void_p(f8.data_ptr() + 8 * (3 * nb + o)),
-                                                       dzv.act(), None, None, acc, sp), "bn_silu_bwd " + hd.prefix)
-                        self._count(2, "bn_bwd (reduce, apply) %s c=%d px=%d" % (hd.prefix, hd.c, npx), "bn_silu_bwd",
-                                    2.0 * npx * hd.c * (3 + (4 if hd.up else 0)))
+                    capi.check(L.yb200_bn_silu_bwd(zv.act(), hd.out.gact(), None, hd.up.gact() if hd.up else None, pf(self.flat_scale, o),
+                                                   pf(self.flat_shift, o), pf(self.flat_mean, o), pf(self.flat_invstd, o),
+                                                   ctypes.c_void_p(f8.data_ptr() + 8 * (2 * nb + o)), ctypes.c_void_p(f8.data_ptr() + 8 * (3 * nb + o)),
+                                                   dzv.act(), None, None, acc, sp), "bn_silu_bwd " + hd.prefix)
+                    self._count(2, "bn_bwd (reduce, apply) %s c=%d px=%d" % (hd.prefix, hd.c, npx), "bn_silu_bwd",
+                                2.0 * npx * hd.c * (3 + (4 if hd.up else 0)))
                     if hd.residual is not None:
                         pending_res[(id(hd.residual.buf), hd.residual.off)] = hd.out
                 dz = dzb.view()
@@ -960,19 +859,16 @@ class YoloxEngine:
                     add = self._grad_target(op.x)
                     assert not (res is not None and add is not None), "residual + fan-out on the same activation"
                     addend = res.gact() if res is not None else (add.gact() if add is not None else None)
-                    nseg = self._dgrad(dz.act(), op.w_dgrad, op.x, addend, op.ksize, op.stride, ("conv", id(op), None), "dgrad " + op.prefixes[0])
-                    self._count(4 if op.stride == 2 else 1, "dgrad%s %s %s" % (" +bn_stats" if nseg else "", op.prefixes[0], self._desc(op)),
-                                "dgrad (conv_gemm, BN-bwd statistics fused where possible)", *self._alg_conv(op))
+                    capi.check(L.yb200_conv2d_dgrad(dz.act(), capi.ptr(op.w_dgrad), op.x.gact(), addend, op.ksize, op.stride, sp), "dgrad " + op.prefixes[0])
+                    self._count(1, "dgrad %s %s" % (op.prefixes[0], self._desc(op)), "dgrad (conv_gemm)", *self._alg_conv(op))
         # BatchNorm weight / bias gradients of the whole range out of the fp64 accumulators: one launch (the per-layer kernels left them there)
         heads = [hd for op in self.ops[lo_i:hi_i] if isinstance(op, ConvOp) for hd in op.heads]
         if heads:
             b0, b1 = min(hd.bn_off for hd in heads), max(hd.bn_off + hd.c for hd in heads)
             assert b1 - b0 == sum(hd.c for hd in heads), "BatchNorm channels of an op range are one run of the flat statistics buffers"
-            raw = self._bn_raw if (self._fuse_active and self._bn_raw is not None) else None
             i4 = lambda t: ctypes.c_void_p(t.data_ptr() + 4 * b0)
             capi.check(L.yb200_bn_param_grads(ctypes.c_void_p(f8.data_ptr() + 8 * (2 * nb + b0)), ctypes.c_void_p(f8.data_ptr() + 8 * (3 * nb + b0)), b1 - b0,
-                                              i4(self.bn_goff), i4(self.bn_boff), capi.ptr(self.flat_grad), i4(self.flat_mean), i4(self.flat_invstd),
-                                              ctypes.c_void_p(raw.data_ptr() + b0) if raw is not None else None, acc, sp), "bn_param_grads")
+                                              i4(self.bn_goff), i4(self.bn_boff), capi.ptr(self.flat_grad), acc, sp), "bn_param_grads")
             self._count(1, "bn param grads of %d layers" % len(heads), "bn_silu_bwd")
         if self.overlap_wgrad:
             torch.cuda.current_stream().wait_stream(self._side)  # join: gradients are complete when backward() returns

@@ -567,35 +567,17 @@ class YOLOX(nn.Module):
         if same and all(i.is_cuda for i in imgs):
             images_dst.copy_(torch.stack(imgs))
         elif same:
-            # host images: one H2D copy of the whole batch.  If the images already are consecutive slices of one pinned
-            # tensor (a collated batch) it is used as is; otherwise they are gathered into a persistent pinned staging buffer.
+            # host images: one H2D copy of the whole batch if the images are consecutive slices of one pinned tensor (a collated batch)
             nbytes = imgs[0].numel()
             base = imgs[0]
             contiguous_run = base.is_pinned() and all(i.is_contiguous() and i.data_ptr() == base.data_ptr() + k * nbytes for k, i in enumerate(imgs))
             if contiguous_run:
                 images_dst.copy_(torch.as_strided(base, (len(imgs), 3, hp, wp), (nbytes, hp * wp, wp, 1)), non_blocking=True)
-            elif all(i.is_pinned() and i.is_contiguous() for i in imgs):
-                for k, im in enumerate(imgs):  # separately allocated pinned images: one asynchronous DMA each, no host-side gather
-                    images_dst[k].copy_(im, non_blocking=True)
             else:
-                # what a detectron2 dataloader hands over: a list of separately allocated pageable tensors: by default one asynchronous copy per
-                # image straight from pageable memory (the driver stages it); a pinned staging buffer can be filled by a thread pool or torch.stack.
-                mode = os.environ.get("YB200_GATHER", "direct")  # direct | threads | stack (A/B knob)
-                if mode == "direct":  # one cudaMemcpyAsync per pageable image: the driver stages each through its own pinned buffers
-                    for k, im in enumerate(imgs):
-                        images_dst[k].copy_(im, non_blocking=True)
-                else:
-                    if getattr(eng, "_stage", None) is None:
-                        eng._stage = torch.empty(images_dst.shape, dtype=torch.uint8).pin_memory()
-                        eng._stage_evt = torch.cuda.Event()
-                    else:
-                        eng._stage_evt.synchronize()  # the previous DMA out of the staging buffer has finished
-                    if mode == "threads":
-                        self._gather(imgs, eng._stage)
-                    else:
-                        torch.stack(imgs, out=eng._stage)
-                    images_dst.copy_(eng._stage, non_blocking=True)
-                    eng._stage_evt.record()
+                # separately allocated images (what a detectron2 dataloader hands over): one asynchronous copy each, no host-side gather;
+                # the driver stages pageable memory through its own pinned buffers
+                for k, im in enumerate(imgs):
+                    images_dst[k].copy_(im, non_blocking=True)
         else:
             if not getattr(eng, "device_pad", True):  # a plan that reads images_u8 as is: the padding value goes in here
                 images_dst.fill_(int(round(self.padded_value)))
@@ -604,21 +586,6 @@ class YOLOX(nn.Module):
         hw_dst.copy_(torch.tensor([[i.shape[-2], i.shape[-1]] for i in imgs], dtype=torch.int32), non_blocking=True)
         if training:
             self._stage_labels(batched_inputs, labels_dst)
-
-    def _gather(self, imgs, stage):
-        """stage[k] = imgs[k] on a small thread pool (Tensor.copy_ releases the GIL: the memcpys run in parallel)"""
-        pool = getattr(self, "_gather_pool", None)
-        if pool is None:
-            from concurrent.futures import ThreadPoolExecutor
-            pool = self._gather_pool = ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1), thread_name_prefix="yb200-gather")
-        n = len(imgs)
-        chunk = max(1, (n + 7) // 8)
-
-        def work(lo):
-            for k in range(lo, min(lo + chunk, n)):
-                stage[k].copy_(imgs[k])
-
-        list(pool.map(work, range(0, n, chunk)))
 
     def _stage_labels(self, batched_inputs, labels_dst):
         """[B, max_boxes, 5] = (cls, cx, cy, w, h), zero padded (yolox.py:150-162, BoxModeMy XYXY_ABS -> cxcywh boxes.py:547-551).

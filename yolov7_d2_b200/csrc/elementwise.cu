@@ -598,32 +598,51 @@ spp_pool_tiled_kernel(View x, View o5, View o9, View o13, uint8_t* __restrict__ 
   }
 }
 
-// backward for the same maps: one block per (CG channels, image) scatters the three pooled gradients to their argmax positions in SHARED memory
-// (fp32 atomics on a [hw][CG] plane) and adds the identity-branch gradient -- no scratch plane in HBM, no global atomics
+// backward for the same maps: one block per (CG channels, image) routes the three pooled gradients to their argmax positions in a SHARED
+// [hw][CG] fp32 plane that starts as the identity-branch gradient -- no scratch plane in HBM, no atomics.  One thread owns each (row, channel) of
+// the plane and adds the gradients that land there in a fixed order (branch 5, 9, 13, then source pixel): the sums, and so the bf16 results, are
+// the same in every run (shared-memory atomics added them in an order that depended on warp scheduling).
 template <int CG>
 __global__ void __launch_bounds__(256)
 spp_pool_bwd_tiled_kernel(View d0, View d5, View d9, View d13, const uint8_t* __restrict__ arg, View dx) {
   pdl_sync();
-  extern __shared__ float sacc[];  // [hw][CG]
+  extern __shared__ float sacc[];  // [hw][CG] fp32 gradient plane, then the [hw][CG] bf16 gradients and argmax codes of one branch
   const int hw = dx.h * dx.w;
   const int cg = blockIdx.x * CG;
   const int b = blockIdx.y;
   const int total = hw * CG;
+  __nv_bfloat16* const sgrad = reinterpret_cast<__nv_bfloat16*>(sacc + total);
+  uint8_t* const scode = reinterpret_cast<uint8_t*>(sgrad + total);
   for (int e = threadIdx.x; e < total; e += blockDim.x) {
     const int ch = e % CG, p = e / CG;
     sacc[e] = __bfloat162float(d0.p[(static_cast<size_t>(b) * hw + p) * d0.pitch + cg + ch]);
   }
-  __syncthreads();
 #pragma unroll 1
   for (int j = 0; j < 3; ++j) {
     const View& d = j == 0 ? d5 : (j == 1 ? d9 : d13);
     const uint8_t* a = arg + (static_cast<size_t>(j) * dx.n + b) * hw * dx.c + cg;
+    __syncthreads();  // the previous branch is done with sgrad / scode
     for (int e = threadIdx.x; e < total; e += blockDim.x) {
       const int ch = e % CG, p = e / CG;
-      const float g = __bfloat162float(d.p[(static_cast<size_t>(b) * hw + p) * d.pitch + cg + ch]);
-      const int code = a[static_cast<size_t>(p) * dx.c + ch];
-      const int q = p + (code / 13 - 6) * dx.w + (code % 13 - 6);
-      atomicAdd(&sacc[q * CG + ch], g);
+      sgrad[e] = d.p[(static_cast<size_t>(b) * hw + p) * d.pitch + cg + ch];
+      scode[e] = a[static_cast<size_t>(p) * dx.c + ch];
+    }
+    __syncthreads();
+    // thread (y, ch) scans the source rows whose windows reach row y (pool 5 / 9 / 13: the argmax lies within 2 / 4 / 6 rows) and adds the
+    // gradients whose argmax lies in row y
+    const int r = 2 + 2 * j;
+    for (int t = threadIdx.x; t < dx.h * CG; t += blockDim.x) {
+      const int ch = t % CG, y = t / CG;
+      const int y0 = max(y - r, 0), y1 = min(y + r, dx.h - 1);
+      for (int py = y0; py <= y1; ++py) {
+        for (int px = 0; px < dx.w; ++px) {
+          const int p = py * dx.w + px;
+          const int code = scode[p * CG + ch];
+          const int dy = code / 13 - 6;
+          if (py + dy != y) continue;
+          sacc[(p + dy * dx.w + (code % 13 - 6)) * CG + ch] += __bfloat162float(sgrad[p * CG + ch]);
+        }
+      }
     }
   }
   __syncthreads();
@@ -880,8 +899,9 @@ extern "C" int yb200_spp_pool_bwd(const yb200_act* d0, const yb200_act* d5, cons
   cudaStream_t st = as_stream(stream);
   const long long elems = 1LL * dx->n * dx->h * dx->w * dx->c;
   constexpr int kCg = 16;
-  const size_t tiled_smem = static_cast<size_t>(dx->h) * dx->w * kCg * sizeof(float);
-  if (dx->c % kCg == 0 && tiled_smem <= 200 * 1024) {  // same condition as the forward: the argmax codes stay inside the map
+  // fp32 gradient plane + one branch's bf16 gradients and argmax codes
+  const size_t tiled_smem = static_cast<size_t>(dx->h) * dx->w * kCg * (sizeof(float) + sizeof(__nv_bfloat16) + 1);
+  if (dx->c % kCg == 0 && tiled_smem <= 200 * 1024) {  // every map the forward pools in shared memory (8 B per element) fits here
     static PerDevice<size_t> smem_set_dev(48 * 1024);
     size_t& smem_set = smem_set_dev.cur();
     if (tiled_smem > smem_set) {

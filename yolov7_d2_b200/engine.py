@@ -329,8 +329,14 @@ class YoloxEngine:
                                     idx[e * co:(e + 1) * co, f * ci_pad:f * ci_pad + ci_real, :, t] = ((c_i * ci_real + ci_i) * 3 + kh_i) * 3 + kw
                                     msk[e * co:(e + 1) * co, f * ci_pad:f * ci_pad + ci_real, :, t] = 1.0
                     op.exp_idx, op.exp_mask = idx.to(dev), msk.to(dev)
-                    op.exp_valid = torch.nonzero(msk.flatten()).flatten().to(dev)       # positions of W' that map to a real weight
-                    op.exp_target = idx.flatten()[op.exp_valid.cpu()].to(dev)            # ... and the flat index of that weight
+                    valid = torch.nonzero(msk.flatten()).flatten()                      # positions of W' that map to a real weight
+                    target = idx.flatten()[valid]                                         # ... and the flat index of that weight
+                    # every real weight appears once per output pixel e of the group: row w of fold_pos lists the g positions of weight w in
+                    # ascending order, so the fold is a fixed-order sum (an index_add_ adds them with atomics, in an order that varies run to run)
+                    order = torch.sort(target, stable=True).indices
+                    assert torch.equal(target[order], torch.arange(co * ci_real * 9).repeat_interleave(g)), "stem expansion"
+                    op.fold_pos = valid[order].to(dev)
+                    op.fold_parts = torch.empty(co * ci_real * 9, g, device=dev)  # gathered once per step; allocated here, not on the side stream
                     op.w_exp = torch.zeros(g * co, g * ci_pad, 3, 3, device=dev)         # fp32 OIHW of the grouped convolution
                     op.g_exp = torch.zeros_like(op.w_exp)
                     op.w_fwd = torch.empty(g * co, kk, g * ci_pad, dtype=torch.bfloat16, device=dev)
@@ -739,9 +745,13 @@ class YoloxEngine:
             capi.check(L.yb200_conv2d_wgrad_grouped(ctypes.byref(xg), ctypes.byref(dzg), 3, 1, 4 * op.cin_pad, 4, capi.ptr(op.g_exp), 0, capi.ptr(self.ws),
                                                     ctypes.c_int64(self.ws_bytes), capi.stream_ptr()), "wgrad stem (grouped)")
             g = op.g_dst.reshape(-1)
-            if not acc:
-                g.zero_()
-            g.index_add_(0, op.exp_target, op.g_exp.reshape(-1)[op.exp_valid])  # every real weight appears in several (e, f, t) positions
+            parts = op.fold_parts  # every real weight appears in several (e, f, t) positions
+            torch.index_select(op.g_exp.reshape(-1), 0, op.fold_pos, out=parts.view(-1))
+            for i in range(parts.shape[1]):  # added one position at a time, in ascending position order
+                if i == 0 and not acc:
+                    g.copy_(parts[:, 0])
+                else:
+                    g.add_(parts[:, i])
 
         if self.overlap_wgrad:
             main = torch.cuda.current_stream()

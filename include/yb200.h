@@ -140,7 +140,10 @@ int yb200_bn_param_grads(double* acc_dgamma, double* acc_dbeta, int c, const int
  * argmax (may be NULL): uint8 [3][n][h][w][c] window offsets for the backward.                                */
 int yb200_spp_pool(const yb200_act* x, const yb200_act* o5, const yb200_act* o9, const yb200_act* o13, uint8_t* argmax,
                    void* stream);
-/* dx = d0 + maxpool-backward(d5, d9, d13);  scratch: fp32 [n*h*w*c].                                           */
+/* dx = d0 + maxpool-backward(d5, d9, d13);  scratch: fp32 [n*h*w*c].
+ * Bit-reproducible only on the shared-memory path (c % 16 == 0 and h*w*16*7 B <= 200 KiB, i.e. maps up to 42x42 for a square map): it adds
+ * the gradients routed to each input in a fixed order.  Other shapes scatter them with fp32 atomics into `scratch`, in an order that can
+ * change from run to run, so the last bits of dx can too.                                                         */
 int yb200_spp_pool_bwd(const yb200_act* d0, const yb200_act* d5, const yb200_act* d9, const yb200_act* d13,
                        const uint8_t* argmax, float* scratch, const yb200_act* dx, void* stream);
 int yb200_copy_view(const yb200_act* src, const yb200_act* dst, void* stream);

@@ -158,20 +158,20 @@ def test_backward_against_oracle(step, cuda):
 
 
 def test_second_step_is_reproducible(step):
-    """a second identical step reproduces the same result (no stale accumulators; fp64 atomics are the only reordering)"""
+    """a second identical step reproduces the first bit for bit: no stale accumulators, and every sum whose order could change from run to
+    run is fixed-order (the SPP backward, the stem's weight-gradient fold).  The BatchNorm statistics still add per-CTA fp32 partials with
+    fp64 atomics in a varying order; fp64 carries 29 more significand bits than the partials, so the sum of a channel's few hundred partials
+    of similar magnitude is exact and its order does not change the bits either."""
     eng = step["eng"]
-    eng.load_state_dict(step["sd0"])
-    eng.train_step()
-    torch.cuda.synchronize()
-    g1, l1 = eng.flat_grad.clone(), eng.losses.clone()
-    eng.load_state_dict(step["sd0"])
-    eng.train_step()
-    torch.cuda.synchronize()
-    assert torch.allclose(l1, eng.losses, rtol=1e-6)
-    rel = (g1 - eng.flat_grad).abs().max() / g1.abs().max()
-    # block reductions run in a fixed order; only fp64 atomics are unordered (1e-16) -- but a single flipped bf16 rounding is
-    # amplified by the backward chain of BatchNorms, so allow a small residue rather than demanding bit equality
-    assert rel <= 2e-3, rel.item()
+    names = ("losses", "outputs", "flat_grad", "flat_rm", "flat_rv", "flat_mean", "flat_invstd")
+    runs = []
+    for _ in range(2):
+        eng.load_state_dict(step["sd0"])
+        eng.train_step()
+        torch.cuda.synchronize()
+        runs.append({k: getattr(eng, k).clone() for k in names})
+    for k in names:
+        assert torch.equal(runs[0][k], runs[1][k]), k
 
 
 def test_eval_forward_matches_oracle(step):

@@ -3,7 +3,7 @@
 # usage: tools/gpu_suite.sh [group ...]   logs -> profile_out/suite_<group>.log
 mkdir -p profile_out
 groups=("$@")
-[ ${#groups[@]} -eq 0 ] && groups=(conv_fwd fwd_b fwd_c fwd_d fwd_e conv_misc conv_dgrad conv_wgrad elementwise simota nms engine modeling iou fused optim cnx_ops cnx_engine attention detr sparseinst)
+[ ${#groups[@]} -eq 0 ] && groups=(conv_fwd fwd_b fwd_c fwd_d fwd_e conv_misc conv_dgrad conv_wgrad elementwise simota nms engine modeling iou fused optim streams fixed_order cnx_ops cnx_engine attention detr sparseinst)
 for g in "${groups[@]}"; do
   case $g in
     conv_fwd)    sel="tests/test_conv_gpu.py -k 'test_conv_fwd_stats and not 1x320 and not 16x64 and not 8x80x80'" ;;
@@ -21,6 +21,8 @@ for g in "${groups[@]}"; do
     nms)         sel="tests/test_nms_gpu.py" ;;
     modeling)    sel="tests/test_modeling_gpu.py" ;;
     iou)         sel="tests/test_iou_loss_gpu.py" ;;
+    streams)     sel="tests/test_streams_gpu.py" ;;
+    fixed_order) sel="tests/test_fixed_order_gpu.py" ;;
     fused)       sel="tests/test_conv_gpu.py -k fused" ;;
     optim)       sel="tests/test_optim_gpu.py" ;;
     attention)   sel="tests/test_attention_gpu.py tests/test_attention_bwd_gpu.py" ;;

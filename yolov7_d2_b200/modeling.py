@@ -624,11 +624,23 @@ class YOLOX(nn.Module):
         current step is still running; the following `forward(batched_inputs)` with this same list only copies device-to-device into the plan's
         static buffers.  The copies go into the plan's alternate buffers as soon as their previous contents have been consumed.  Optional: forward() alone behaves exactly like the reference (copy, then compute)."""
         eng, imgs, hp, wp = self._plan_for(batched_inputs)
-        if getattr(eng, "_alt", None) is None:
-            eng._alt = (torch.empty_like(eng.images_u8), torch.empty_like(eng.labels), torch.empty_like(eng.hw_valid))
         if self._copy_stream is None:
             self._copy_stream = torch.cuda.Stream(device=self.device)
             self._copy_done = torch.cuda.Event()
+        cur = torch.cuda.current_stream()
+        if getattr(eng, "_alt", None) is None:
+            eng._alt = (torch.empty_like(eng.images_u8), torch.empty_like(eng.labels), torch.empty_like(eng.hw_valid))
+            # the caching allocator may hand these out from blocks that work queued on the current stream still reads or writes (a
+            # temporary freed by the step in flight): the copy stream must not write them before that work is done (once per plan)
+            self._copy_stream.wait_stream(cur)
+        # inputs that live on the device were produced on the caller's stream: read them after it, and keep their memory from being reused
+        # before the copy stream is done with it, so that the caller may drop its references as soon as prefetch() returns.  Host inputs
+        # add no wait: their copies overlap the step in flight.
+        dev_inputs = self._device_inputs(batched_inputs, imgs)
+        if dev_inputs:
+            self._copy_stream.wait_stream(cur)
+            for t in dev_inputs:
+                t.record_stream(self._copy_stream)
         with torch.cuda.stream(self._copy_stream):
             # the alternate buffers were last READ by the device-to-device copy at the head of the step that consumed the previous prefetch
             # (preprocess_image records `_alt_free` there): wait for that, not for the whole step in flight -- the DMA overlaps its kernels
@@ -638,6 +650,16 @@ class YOLOX(nn.Module):
             self._stage_batch(batched_inputs, self.training, eng, imgs, hp, wp, *eng._alt)
             self._copy_done.record(self._copy_stream)
         self._prefetched = (batched_inputs, eng)
+
+    def _device_inputs(self, batched_inputs, imgs):
+        """the caller's CUDA tensors that staging a batch reads: images, and the ground truth when training"""
+        out = [i for i in imgs if i.is_cuda]
+        if self.training:
+            for x in batched_inputs:
+                inst = x.get("instances", x.get("targets"))
+                if inst is not None:
+                    out += [t for t in (inst.gt_boxes.tensor, inst.gt_classes) if t.is_cuda]
+        return out
 
     def preprocess_image(self, batched_inputs, training):
         eng, imgs, hp, wp = self._plan_for(batched_inputs)

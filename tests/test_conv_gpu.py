@@ -37,6 +37,9 @@ SHAPES = [
     (16, 64, 64, 16, 32, 3, 1),    # 512 CTAs: several CTAs resident per SM, more than one wave
     (16, 64, 64, 64, 64, 1, 1),    # 512 single-k-block CTAs (memory-bound 1x1)
     (8, 80, 80, 128, 128, 3, 1),   # 400 CTAs x 18 k-blocks
+    (8, 80, 80, 128, 80, 1, 1),    # prediction convolutions: cls (80 channels) at the stride-8 level ...
+    (8, 20, 20, 128, 80, 1, 1),    # ... and the stride-32 level
+    (8, 40, 40, 128, 16, 1, 1),    # reg + obj, 5 channels padded to 16: 16-channel block of the data gradient
 ]
 
 

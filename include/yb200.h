@@ -378,6 +378,37 @@ int yb200_attention_bwd_dropout(const yb200_act* q, const yb200_act* k, const yb
 int yb200_dropout(const yb200_act* x, const yb200_act* residual, const yb200_act* out, float p_drop, uint32_t seed, float extra_scale,
                   void* stream);
 
+/* ---- mosaic / random_perspective / mixup of the YOLOX training mapper ------------------------------------------------------------------------ */
+/* MyDatasetMapper2.__call__ (yolov7/data/dataset_mapper.py:477-611, mixup :686-767) with random_perspective (data_augment.py:31-102): the host
+ * (yolov7_d2_b200/augment.py) makes the random draws and computes the boxes; these two calls render the pixels of a whole batch.  One descriptor
+ * per sample in DEVICE memory; the sources are HWC uint8 (BGR) images packed in one buffer, the outputs CHW uint8 (the reference's
+ * `img.transpose(2, 0, 1)`, :637-638) packed in another.  Bit-reproducible (no atomics), no host synchronisation.
+ *   yb200_mosaic_warp: mode 1 -- the four tiles cv2.resize'd (INTER_LINEAR) into the 2h x 2w canvas of 114 (:529-566), then
+ *     cv2.warpAffine(canvas, M[:2], (out_w, out_h), borderValue 114) with minv = the inverse of M (data_augment.py:62-74); mode 0 -- a sample
+ *     without mosaic (pool still filling, or mosaic_flag 0): source 0 copied HWC -> CHW.
+ *   yb200_mosaic_mixup: for samples with mode 1 and mix 1, the mixup image (:701-739: resize of source 4 into the in_h x in_w canvas of 114,
+ *     float64 resize to jit_h x jit_w, optional horizontal flip, zero padding, crop at (y_off, x_off)) blended into the output in place,
+ *     (a + b) / 2 truncated (:763-767).  Run it after yb200_mosaic_warp on the same stream.
+ * max_h / max_w bound the output sizes of the batch (they size the grid).                                                                      */
+typedef struct yb200_mosaic_desc {
+  int64_t src_off[5];          /* byte offsets of the sources in `src`: tiles 0-3 (top left, top right, bottom left, bottom right), mixup 4 */
+  int64_t out_off;             /* byte offset of the sample's [3][out_h][out_w] output in `out` */
+  double minv[6];              /* inverse of the 2x3 affine map: output pixel -> canvas pixel */
+  int32_t src_h[5], src_w[5];
+  int32_t tile_h[4], tile_w[4];  /* resized tile size: (int(h0 * s), int(w0 * s)), s = min(h / h0, w / w0) */
+  int32_t rect[16];            /* per tile: canvas rectangle x1a, y1a, x2a, y2a */
+  int32_t pad[8];              /* per tile: padw, padh (canvas position of the tile's pixel (0, 0)) */
+  int32_t in_h, in_w;          /* mosaic size (h, w); the canvas is 2h x 2w */
+  int32_t out_h, out_w;
+  int32_t mode;                /* 0: copy source 0, 1: mosaic */
+  int32_t mix;                 /* 1: blend the mixup image */
+  int32_t mix_h, mix_w;        /* resized mixup source inside the in_h x in_w canvas */
+  int32_t jit_h, jit_w;        /* jittered canvas size */
+  int32_t flip, x_off, y_off, reserved;
+} yb200_mosaic_desc;
+int yb200_mosaic_warp(const yb200_mosaic_desc* table_dev, int n, const uint8_t* src, uint8_t* out, int max_h, int max_w, void* stream);
+int yb200_mosaic_mixup(const yb200_mosaic_desc* table_dev, int n, const uint8_t* src, uint8_t* out, int max_h, int max_w, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

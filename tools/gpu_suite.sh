@@ -3,7 +3,7 @@
 # usage: tools/gpu_suite.sh [group ...]   logs -> profile_out/suite_<group>.log
 mkdir -p profile_out
 groups=("$@")
-[ ${#groups[@]} -eq 0 ] && groups=(conv_fwd fwd_b fwd_c fwd_d fwd_e conv_misc conv_dgrad conv_wgrad elementwise simota nms engine modeling iou fused optim streams fixed_order train_bn cnx_ops cnx_engine attention detr sparseinst)
+[ ${#groups[@]} -eq 0 ] && groups=(conv_fwd fwd_b fwd_c fwd_d fwd_e conv_misc conv_dgrad conv_wgrad elementwise simota nms engine modeling iou fused optim streams fixed_order train_bn mosaic cnx_ops cnx_engine attention detr sparseinst)
 for g in "${groups[@]}"; do
   case $g in
     conv_fwd)    sel="tests/test_conv_gpu.py -k 'test_conv_fwd_stats and not 1x320 and not 16x64 and not 8x80x80'" ;;
@@ -24,6 +24,7 @@ for g in "${groups[@]}"; do
     streams)     sel="tests/test_streams_gpu.py" ;;
     fixed_order) sel="tests/test_fixed_order_gpu.py" ;;
     train_bn)    sel="tests/test_train_bn_gpu.py" ;;
+    mosaic)      sel="tests/test_mosaic_gpu.py" ;;
     fused)       sel="tests/test_conv_gpu.py -k fused" ;;
     optim)       sel="tests/test_optim_gpu.py" ;;
     attention)   sel="tests/test_attention_gpu.py tests/test_attention_bwd_gpu.py" ;;

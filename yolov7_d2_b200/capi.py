@@ -48,6 +48,21 @@ class PackDesc(ctypes.Structure):
                 ("ksize", ctypes.c_int32), ("cout_pad", ctypes.c_int32), ("cin_pad", ctypes.c_int32), ("reserved", ctypes.c_int32)]
 
 
+MOSAIC_MAX_SOURCES = 5  # four tiles and the mixup source
+
+
+class MosaicDesc(ctypes.Structure):
+    """mirror of `yb200_mosaic_desc` (include/yb200.h)"""
+
+    _fields_ = [("src_off", c_i64 * MOSAIC_MAX_SOURCES), ("out_off", c_i64), ("minv", ctypes.c_double * 6),
+                ("src_h", ctypes.c_int32 * MOSAIC_MAX_SOURCES), ("src_w", ctypes.c_int32 * MOSAIC_MAX_SOURCES),
+                ("tile_h", ctypes.c_int32 * 4), ("tile_w", ctypes.c_int32 * 4), ("rect", ctypes.c_int32 * 16), ("pad", ctypes.c_int32 * 8),
+                ("in_h", ctypes.c_int32), ("in_w", ctypes.c_int32), ("out_h", ctypes.c_int32), ("out_w", ctypes.c_int32),
+                ("mode", ctypes.c_int32), ("mix", ctypes.c_int32), ("mix_h", ctypes.c_int32), ("mix_w", ctypes.c_int32),
+                ("jit_h", ctypes.c_int32), ("jit_w", ctypes.c_int32), ("flip", ctypes.c_int32), ("x_off", ctypes.c_int32),
+                ("y_off", ctypes.c_int32), ("reserved", ctypes.c_int32)]
+
+
 def declared_symbols(header_path=HEADER_PATH):
     """Every function the public header declares (used by the CPU test that checks the exports)."""
     with open(header_path) as fh:

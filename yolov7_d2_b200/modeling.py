@@ -623,11 +623,18 @@ class YOLOX(nn.Module):
         """Input-side pipelining (SURVEY.md par.8f rank 2): start the host->device copies of the NEXT batch on a copy stream while the
         current step is still running; the following `forward(batched_inputs)` with this same list only copies device-to-device into the plan's
         static buffers.  The copies go into the plan's alternate buffers as soon as their previous contents have been consumed.  Optional: forward() alone behaves exactly like the reference (copy, then compute)."""
-        eng, imgs, hp, wp = self._plan_for(batched_inputs)
         if self._copy_stream is None:
             self._copy_stream = torch.cuda.Stream(device=self.device)
             self._copy_done = torch.cuda.Event()
         cur = torch.cuda.current_stream()
+        from . import augment  # imports this module
+
+        rendered = set()
+        if augment.has_recipes(batched_inputs):
+            # mosaic recipes are rendered on the copy stream, into memory allocated there: stream order alone protects it
+            with torch.cuda.stream(self._copy_stream):
+                rendered = {id(t) for t in augment.apply_mosaic(batched_inputs)}
+        eng, imgs, hp, wp = self._plan_for(batched_inputs)
         if getattr(eng, "_alt", None) is None:
             eng._alt = (torch.empty_like(eng.images_u8), torch.empty_like(eng.labels), torch.empty_like(eng.hw_valid))
             # the caching allocator may hand these out from blocks that work queued on the current stream still reads or writes (a
@@ -636,7 +643,7 @@ class YOLOX(nn.Module):
         # inputs that live on the device were produced on the caller's stream: read them after it, and keep their memory from being reused
         # before the copy stream is done with it, so that the caller may drop its references as soon as prefetch() returns.  Host inputs
         # add no wait: their copies overlap the step in flight.
-        dev_inputs = self._device_inputs(batched_inputs, imgs)
+        dev_inputs = [t for t in self._device_inputs(batched_inputs, imgs) if id(t) not in rendered]
         if dev_inputs:
             self._copy_stream.wait_stream(cur)
             for t in dev_inputs:
@@ -683,6 +690,10 @@ class YOLOX(nn.Module):
 
     # -- forward ---------------------------------------------------------------------------------
     def forward(self, batched_inputs):
+        from . import augment  # imports this module
+
+        if augment.has_recipes(batched_inputs):  # MosaicMixupMapper output: render the mosaics first (augment.py)
+            augment.apply_mosaic(batched_inputs)
         eng, image_sizes = self.preprocess_image(batched_inputs, self.training)
         if self.training:
             if self._flat_grads:

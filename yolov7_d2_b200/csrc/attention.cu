@@ -583,11 +583,11 @@ attention_bwd_q_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
   }
 }
 
-int check_seq(const yb200_act* a, const char* name) {
-  YB_REQUIRE(a && a->ptr, YB200_ERR_INVALID, "%s: null view", name);
-  YB_REQUIRE(a->n > 0 && a->h == 1 && a->w > 0 && a->c > 0, YB200_ERR_INVALID, "%s: expected a [B][1][L][E] view (got %dx%dx%dx%d)", name, a->n, a->h, a->w, a->c);
-  YB_REQUIRE(a->c % kAttD == 0 && a->c_pitch % 8 == 0 && a->c_off % 8 == 0 && a->c_off + a->c <= a->c_pitch, YB200_ERR_INVALID,
-             "%s: channels (c=%d pitch=%d off=%d): c must be heads x 32", name, a->c, a->c_pitch, a->c_off);
+// a token sequence: a [B][1][L][E] view with E = heads x 32
+int check_tokens(const yb200_act* a, const char* name) {
+  if (const int rc = check_act(a, name)) return rc;
+  YB_REQUIRE(a->h == 1 && a->c % kAttD == 0, YB200_ERR_INVALID, "%s: expected a [B][1][L][heads x 32] view (got %dx%dx%dx%d)", name, a->n, a->h,
+             a->w, a->c);
   return 0;
 }
 
@@ -613,10 +613,10 @@ extern "C" int yb200_attention_fwd_dropout(const yb200_act* q, const yb200_act* 
 static int attention_fwd_impl(const yb200_act* q, const yb200_act* k, const yb200_act* v, const uint8_t* key_padding_mask, float scale,
                               const yb200_act* out, float* lse, float p_drop, uint32_t seed, void* stream) {
   int rc;
-  if ((rc = check_seq(q, "attention_fwd q"))) return rc;
-  if ((rc = check_seq(k, "attention_fwd k"))) return rc;
-  if ((rc = check_seq(v, "attention_fwd v"))) return rc;
-  if ((rc = check_seq(out, "attention_fwd out"))) return rc;
+  if ((rc = check_tokens(q, "attention_fwd q"))) return rc;
+  if ((rc = check_tokens(k, "attention_fwd k"))) return rc;
+  if ((rc = check_tokens(v, "attention_fwd v"))) return rc;
+  if ((rc = check_tokens(out, "attention_fwd out"))) return rc;
   YB_REQUIRE(k->n == q->n && v->n == q->n && out->n == q->n && k->w == v->w && out->w == q->w && k->c == q->c && v->c == q->c && out->c == q->c,
              YB200_ERR_INVALID, "attention_fwd: shapes q %dx%dx%d k %dx%dx%d v %dx%dx%d out %dx%dx%d", q->n, q->w, q->c, k->n, k->w, k->c, v->n, v->w, v->c,
              out->n, out->w, out->c);
@@ -633,13 +633,8 @@ static int attention_fwd_impl(const yb200_act* q, const yb200_act* k, const yb20
   p.out = static_cast<__nv_bfloat16*>(out->ptr);
   p.out_pitch = out->c_pitch; p.out_coff = out->c_off;
   p.lse = lse;
-  static PerDevice<bool> attr_set_dev(false);
-  bool& attr_set = attr_set_dev.cur();
-  if (!attr_set) {
-    YB_CHECK_CUDA(cudaFuncSetAttribute(attention_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttSmem));
-    YB_CHECK_CUDA(cudaFuncSetAttribute(attention_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttSmem));
-    attr_set = true;
-  }
+  static PerDevice<int> smem_limit(0);
+  YB_CHECK_CUDA(raise_smem_limit(smem_limit, kAttSmem, attention_fwd_kernel<false>, attention_fwd_kernel<true>));
   dim3 grid(ceil_div(p.lq, kAttTile), p.heads, q->n);
   if (p.drop.thr24 != 0)
     launch_k(attention_fwd_kernel<true>, grid, kAttThreads, kAttSmem, as_stream(stream), tmQ, tmK, tmV, p);
@@ -675,7 +670,7 @@ static int attention_bwd_impl(const yb200_act* q, const yb200_act* k, const yb20
   const char* names[8] = {"attention_bwd q", "attention_bwd k", "attention_bwd v", "attention_bwd out", "attention_bwd dout", "attention_bwd dq", "attention_bwd dk",
                           "attention_bwd dv"};
   for (int i = 0; i < 8; ++i)
-    if ((rc = check_seq(all[i], names[i]))) return rc;
+    if ((rc = check_tokens(all[i], names[i]))) return rc;
   YB_REQUIRE(lse && workspace, YB200_ERR_INVALID, "attention_bwd: null lse / workspace");
   const yb200_act* qlike[3] = {out, dout, dq};
   for (const yb200_act* t : qlike) YB_REQUIRE(t->n == q->n && t->w == q->w && t->c == q->c, YB200_ERR_INVALID, "attention_bwd: query-side shapes differ");
@@ -697,15 +692,9 @@ static int attention_bwd_impl(const yb200_act* q, const yb200_act* k, const yb20
   p.dq = static_cast<__nv_bfloat16*>(dq->ptr); p.dq_pitch = dq->c_pitch; p.dq_coff = dq->c_off;
   p.dk = static_cast<__nv_bfloat16*>(dk->ptr); p.dk_pitch = dk->c_pitch; p.dk_coff = dk->c_off;
   p.dv = static_cast<__nv_bfloat16*>(dv->ptr); p.dv_pitch = dv->c_pitch; p.dv_coff = dv->c_off;
-  static PerDevice<bool> attr_set_dev(false);
-  bool& attr_set = attr_set_dev.cur();
-  if (!attr_set) {
-    YB_CHECK_CUDA(cudaFuncSetAttribute(attention_bwd_kv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmemKV));
-    YB_CHECK_CUDA(cudaFuncSetAttribute(attention_bwd_q_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmemQ));
-    YB_CHECK_CUDA(cudaFuncSetAttribute(attention_bwd_kv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmemKV));
-    YB_CHECK_CUDA(cudaFuncSetAttribute(attention_bwd_q_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBwdSmemQ));
-    attr_set = true;
-  }
+  static PerDevice<int> kv_limit(0), q_limit(0);
+  YB_CHECK_CUDA(raise_smem_limit(kv_limit, kBwdSmemKV, attention_bwd_kv_kernel<false>, attention_bwd_kv_kernel<true>));
+  YB_CHECK_CUDA(raise_smem_limit(q_limit, kBwdSmemQ, attention_bwd_q_kernel<false>, attention_bwd_q_kernel<true>));
   cudaStream_t st = as_stream(stream);
   const long long rows = 1LL * q->n * q->w * p.heads;
   launch_k(attention_bwd_prep_kernel, static_cast<int>((rows + 255) / 256), 256, 0, st, static_cast<const __nv_bfloat16*>(out->ptr), out->c_pitch, out->c_off,
@@ -758,9 +747,9 @@ __global__ void dropout_bf16_kernel(const __nv_bfloat16* __restrict__ x, int x_p
 extern "C" int yb200_dropout(const yb200_act* x, const yb200_act* residual, const yb200_act* out, float p_drop, uint32_t seed, float extra_scale,
                              void* stream) {
   int rc;
-  if ((rc = check_seq(x, "dropout x"))) return rc;
-  if ((rc = check_seq(out, "dropout out"))) return rc;
-  if (residual && (rc = check_seq(residual, "dropout residual"))) return rc;
+  if ((rc = check_tokens(x, "dropout x"))) return rc;
+  if ((rc = check_tokens(out, "dropout out"))) return rc;
+  if (residual && (rc = check_tokens(residual, "dropout residual"))) return rc;
   YB_REQUIRE(out->n == x->n && out->w == x->w && out->c == x->c && (!residual || (residual->n == x->n && residual->w == x->w && residual->c == x->c)),
              YB200_ERR_INVALID, "dropout: shapes differ");
   YB_REQUIRE(1LL * x->n * x->w * x->c < (1LL << 32), YB200_ERR_UNSUPPORTED, "dropout: more than 2^32 elements");

@@ -36,13 +36,8 @@ static int launch_conv_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
   if (pst > kMaxStagesP) pst = kMaxStagesP;
   if (pst < 2) pst = 2;
   const int smem = pst * kbs * Cfg::kStageBytes + 1024 + fixed;
-  static PerDevice<int> max_set_p_dev(0);
-  int& max_set_p = max_set_p_dev.cur();
-  if (smem > max_set_p) {
-    YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_persistent_kernel<BN, BK, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    YB_CHECK_CUDA(cudaFuncSetAttribute(conv_gemm_persistent_kernel<BN, BK, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    max_set_p = smem;
-  }
+  static PerDevice<int> smem_limit(0);
+  YB_CHECK_CUDA(raise_smem_limit(smem_limit, smem, conv_gemm_persistent_kernel<BN, BK, false>, conv_gemm_persistent_kernel<BN, BK, true>));
   int groups = (occ * sm_count()) / n_tiles;
   if (groups < 1) groups = 1;
   if (groups > m_tiles) groups = m_tiles;
@@ -73,12 +68,11 @@ static int pick_block_k(int c) { return c % 64 == 0 ? 64 : (c % 32 == 0 ? 32 : (
 // the epilogue and spills
 static int pick_block_n(int c) { return c > 64 ? 128 : (c > 32 ? 64 : (c > 16 ? 32 : 16)); }
 
-static int check_act(const yb200_act* a, const char* name) {
-  YB_REQUIRE(a != nullptr && a->ptr != nullptr, YB200_ERR_INVALID, "%s: null view", name);
-  YB_REQUIRE(a->n > 0 && a->h > 0 && a->w > 0 && a->c > 0, YB200_ERR_INVALID, "%s: empty extent", name);
-  YB_REQUIRE(a->c % 8 == 0 && a->c_pitch % 8 == 0 && a->c_off % 8 == 0 && a->c_off + a->c <= a->c_pitch, YB200_ERR_INVALID,
-             "%s: channels (c=%d pitch=%d off=%d) must be multiples of 8 with off+c<=pitch", name, a->c, a->c_pitch, a->c_off);
-  return 0;
+// check_act with the message prefix "<entry point> <argument>"
+static int check_arg(const yb200_act* a, const char* who, const char* arg) {
+  char name[96];
+  snprintf(name, sizeof(name), "%s %s", who, arg);
+  return check_act(a, name);
 }
 
 // fill the forward-style tap table (reads input pixel  stride*o + k - pad)
@@ -108,13 +102,63 @@ static int fill_fwd_taps(ConvTap* taps, const yb200_act& x, int ksize, int strid
   return nt;
 }
 
-static void set_out_view(ConvGemmParams& p, const yb200_act& o) {
+// Output geometries: each returns a zeroed parameter block with the output set.
+// 16-bit NHWC view
+static ConvGemmParams out_view(const yb200_act& o) {
+  ConvGemmParams p;
+  memset(&p, 0, sizeof(p));
   p.out = static_cast<__nv_bfloat16*>(o.ptr) + o.c_off;
   p.out_sw = o.c_pitch;
   p.out_sh = 1LL * o.c_pitch * o.w;
   p.out_sn = 1LL * o.c_pitch * o.w * o.h;
   p.out_sc = 1;
   p.out_mh = 1; p.out_mw = 1;
+  return p;
+}
+// fp32 [B, A, C] rows: pixel (y, x) of a w-wide grid is row a_off + y * w + x, its channels start at column c_off
+static ConvGemmParams out_rows_f32(float* out, int w, int a_total, int a_off, int c_total, int c_off) {
+  ConvGemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.out = out + 1LL * a_off * c_total + c_off;
+  p.out_sn = 1LL * a_total * c_total;
+  p.out_sh = 1LL * w * c_total;
+  p.out_sw = c_total;
+  p.out_sc = 1;
+  p.out_mh = 1; p.out_mw = 1;
+  return p;
+}
+// fp32 NCHW [n][cout][h][w], h * w < 2^31
+static ConvGemmParams out_nchw_f32(float* out, int cout, int h, int w) {
+  ConvGemmParams p;
+  memset(&p, 0, sizeof(p));
+  const long long hw = 1LL * h * w;
+  p.out = out;                 // element (n, y, x, c) at n*cout*hw + c*hw + y*w + x: lanes (pixels) write consecutive floats per channel
+  p.out_sn = 1LL * cout * hw;
+  p.out_sh = w;
+  p.out_sw = 1;
+  p.out_sc = static_cast<int>(hw);
+  p.out_mh = 1; p.out_mw = 1;
+  return p;
+}
+// fp32 NHWC [n][h][w][pitch]
+static ConvGemmParams out_nhwc_f32(float* out, int pitch, int h, int w) {
+  ConvGemmParams p;
+  memset(&p, 0, sizeof(p));
+  p.out = out;
+  p.out_sw = pitch;
+  p.out_sh = 1LL * pitch * w;
+  p.out_sn = 1LL * pitch * w * h;
+  p.out_sc = 1;
+  p.out_mh = 1; p.out_mw = 1;
+  return p;
+}
+
+// residual added in the epilogue, a 16-bit NHWC view of the output's shape
+static void set_addend(ConvGemmParams& p, const yb200_act* a) {
+  p.addend = static_cast<const __nv_bfloat16*>(a->ptr) + a->c_off;
+  p.add_sw = a->c_pitch;
+  p.add_sh = 1LL * a->c_pitch * a->w;
+  p.add_sn = 1LL * a->c_pitch * a->w * a->h;
 }
 
 static void set_tiles(ConvGemmParams& p, int n, int h, int w) {
@@ -248,38 +292,44 @@ extern "C" int yb200_pack_conv_weight_scaled(const float* w_oihw, const float* c
 // after plane 0 in the same NHWC buffer and the weight matrix is [rows][plane 0 taps | plane 1 taps | plane 2 taps].  The product keeps every
 // term x_i * w_j with i + j < planes (the dropped ones are below 2^-8planes relative) as extra taps of the SAME implicit GEMM -- one fp32
 // accumulator, no extra kernel: 3 taps per spatial tap for two planes, 6 for three.
-static int conv_fwd_common(const yb200_act* x, const void* w_fwd, int cout, int ksize, int stride, ConvGemmParams& p,
-                           cudaStream_t st, int lo_delta = 0, int planes = 1, int group = 0) {
-  YB_REQUIRE(w_fwd != nullptr, YB200_ERR_INVALID, "conv fwd: null weights");
+static void expand_split_taps(ConvGemmParams& p, int c, int lo_delta, int planes) {
+  const int nt = p.num_taps;
+  const int plane_kb = nt * c;
+  int terms[6][2], nterm = 0;  // (activation plane, weight plane), largest products first
+  for (int sum = 0; sum < planes; ++sum)
+    for (int i = 0; i <= sum; ++i) { terms[nterm][0] = i; terms[nterm][1] = sum - i; ++nterm; }
+  for (int t = nt - 1; t >= 0; --t) {
+    const ConvTap b = p.taps[t];
+    for (int q = 0; q < nterm; ++q) {
+      ConvTap e = b;
+      e.c0 = b.c0 + terms[q][0] * lo_delta;
+      e.kb = b.kb + terms[q][1] * plane_kb;
+      p.taps[nterm * t + q] = e;
+    }
+  }
+  p.num_taps = nterm * nt;
+}
+
+// The launch shared by the forward entry points (`who` names the entry point in messages).  The weight matrix has `w_rows` rows: cout, or
+// n * cout with one matrix per image (p.b_img_rows).
+static int conv_fwd_common(const char* who, const yb200_act* x, const void* w_fwd, long long w_rows, int cout, int ksize, int stride,
+                           ConvGemmParams& p, cudaStream_t st, int lo_delta = 0, int planes = 1, int group = 0) {
+  YB_REQUIRE(w_fwd != nullptr, YB200_ERR_INVALID, "%s: null weights", who);
   YB_REQUIRE((ksize == 1 && stride == 1) || (ksize == 2 && stride == 2) || (ksize == 3 && (stride == 1 || stride == 2)), YB200_ERR_UNSUPPORTED,
-             "conv fwd: ksize=%d stride=%d not implemented", ksize, stride);
+             "%s: ksize=%d stride=%d not implemented", who, ksize, stride);
   const int bk = pick_block_k(x->c);
-  YB_REQUIRE(bk != 0, YB200_ERR_UNSUPPORTED, "conv fwd: input channels %d must be a multiple of 16", x->c);
+  YB_REQUIRE(bk != 0, YB200_ERR_UNSUPPORTED, "%s: input channels %d must be a multiple of 16", who, x->c);
   const int bn = pick_block_n(cout);
   const int oh = x->h / stride, ow = x->w / stride;
   set_tiles(p, x->n, oh, ow);
   p.num_taps = fill_fwd_taps(p.taps, *x, ksize, stride, x->c);
   long long kcols = 1LL * p.num_taps * x->c;
   if (lo_delta > 0) {
-    YB_REQUIRE(planes == 2 || planes == 3, YB200_ERR_INVALID, "conv fwd (split): %d planes", planes);
+    YB_REQUIRE(planes == 2 || planes == 3, YB200_ERR_INVALID, "%s: %d planes", who, planes);
     YB_REQUIRE(lo_delta % 8 == 0 && x->c_off + (planes - 1) * lo_delta + x->c <= x->c_pitch, YB200_ERR_INVALID,
-               "conv fwd (split): plane %d [%d, %d) outside the channel pitch %d", planes - 1, x->c_off + (planes - 1) * lo_delta,
+               "%s: plane %d [%d, %d) outside the channel pitch %d", who, planes - 1, x->c_off + (planes - 1) * lo_delta,
                x->c_off + (planes - 1) * lo_delta + x->c, x->c_pitch);
-    const int nt = p.num_taps;
-    const int plane_kb = nt * x->c;
-    int terms[6][2], nterm = 0;  // (activation plane, weight plane), largest products first
-    for (int sum = 0; sum < planes; ++sum)
-      for (int i = 0; i <= sum; ++i) { terms[nterm][0] = i; terms[nterm][1] = sum - i; ++nterm; }
-    for (int t = nt - 1; t >= 0; --t) {
-      const ConvTap b = p.taps[t];
-      for (int q = 0; q < nterm; ++q) {
-        ConvTap e = b;
-        e.c0 = b.c0 + terms[q][0] * lo_delta;
-        e.kb = b.kb + terms[q][1] * plane_kb;
-        p.taps[nterm * t + q] = e;
-      }
-    }
-    p.num_taps = nterm * nt;
+    expand_split_taps(p, x->c, lo_delta, planes);
     kcols *= planes;
   }
   p.cin_blocks = x->c / bk;
@@ -300,213 +350,147 @@ static int conv_fwd_common(const yb200_act* x, const void* w_fwd, int cout, int 
   CUtensorMap tmA, tmB;
   int rc = make_act_map(&tmA, *x, stride == 2, bk, tw, th, tn);
   if (rc) return rc;
-  rc = make_mat_map(&tmB, w_fwd, cout, kcols, bn, bk);
+  rc = make_mat_map(&tmB, w_fwd, w_rows, kcols, bn, bk);
   if (rc) return rc;
   dim3 grid(p.tiles_w * p.tiles_h * p.tiles_n, ceil_div(cout, bn));
   return launch_conv(bn, bk, tmA, tmB, p, grid, st);
 }
 
-static int conv2d_fwd_impl(const yb200_act* x, const void* w_fwd, const yb200_act* z, int ksize, int stride, double* stat_sum, double* stat_sqsum,
-                           int stat_fold, void* stream);
+// checks shared by the forward entry points with a 16-bit NHWC output: the views, the stride, output grid = input grid / stride, and an
+// optional residual of the output's shape
+static int check_fwd(const char* who, const yb200_act* x, const yb200_act* out, const char* out_name, const yb200_act* residual, int stride) {
+  int rc;
+  if ((rc = check_arg(x, who, "x"))) return rc;
+  if ((rc = check_arg(out, who, out_name))) return rc;
+  if (residual && (rc = check_arg(residual, who, "residual"))) return rc;
+  YB_REQUIRE(stride == 1 || stride == 2, YB200_ERR_UNSUPPORTED, "%s: stride %d", who, stride);
+  YB_REQUIRE(out->n == x->n && out->h * stride == x->h && out->w * stride == x->w, YB200_ERR_INVALID,
+             "%s: output %dx%dx%d does not match input %dx%dx%d / stride %d", who, out->n, out->h, out->w, x->n, x->h, x->w, stride);
+  YB_REQUIRE(!residual || same_shape(residual, out), YB200_ERR_INVALID, "%s: residual shape mismatch", who);
+  return 0;
+}
+
+static int conv2d_fwd_impl(const char* who, const yb200_act* x, const void* w_fwd, const yb200_act* z, int ksize, int stride, double* stat_sum,
+                           double* stat_sqsum, int stat_fold, void* stream) {
+  int rc;
+  if ((rc = check_fwd(who, x, z, "z", nullptr, stride))) return rc;
+  YB_REQUIRE((stat_sum == nullptr) == (stat_sqsum == nullptr), YB200_ERR_INVALID, "%s: pass both or neither stat buffer", who);
+  ConvGemmParams p = out_view(*z);
+  p.epi_mode = stat_sum ? EPI_F16_STATS : EPI_F16;
+  p.stat_sum = stat_sum;
+  p.stat_sq = stat_sqsum;
+  p.stat_fold = stat_fold;
+  return conv_fwd_common(who, x, w_fwd, z->c, z->c, ksize, stride, p, as_stream(stream), 0, 1, stat_fold > 0 ? z->c / stat_fold : 0);
+}
 
 extern "C" int yb200_conv2d_fwd(const yb200_act* x, const void* w_fwd, const yb200_act* z, int ksize, int stride,
                                 double* stat_sum, double* stat_sqsum, void* stream) {
-  return conv2d_fwd_impl(x, w_fwd, z, ksize, stride, stat_sum, stat_sqsum, 0, stream);
+  return conv2d_fwd_impl("conv2d_fwd", x, w_fwd, z, ksize, stride, stat_sum, stat_sqsum, 0, stream);
 }
 
 extern "C" int yb200_conv2d_fwd_fold(const yb200_act* x, const void* w_fwd, const yb200_act* z, int ksize, int stride, double* stat_sum,
                                      double* stat_sqsum, int stat_fold, void* stream) {
   YB_REQUIRE(stat_fold > 0 && z && z->c % stat_fold == 0, YB200_ERR_INVALID, "conv2d_fwd_fold: output channels must be a multiple of stat_fold");
-  return conv2d_fwd_impl(x, w_fwd, z, ksize, stride, stat_sum, stat_sqsum, stat_fold, stream);
-}
-
-static int conv2d_fwd_impl(const yb200_act* x, const void* w_fwd, const yb200_act* z, int ksize, int stride, double* stat_sum, double* stat_sqsum,
-                           int stat_fold, void* stream) {
-  int rc;
-  if ((rc = check_act(x, "conv2d_fwd x"))) return rc;
-  if ((rc = check_act(z, "conv2d_fwd z"))) return rc;
-  YB_REQUIRE(stride == 1 || stride == 2, YB200_ERR_UNSUPPORTED, "conv2d_fwd: stride %d", stride);
-  YB_REQUIRE(z->n == x->n && z->h * stride == x->h && z->w * stride == x->w, YB200_ERR_INVALID,
-             "conv2d_fwd: output %dx%dx%d does not match input %dx%dx%d / stride %d", z->n, z->h, z->w, x->n, x->h, x->w, stride);
-  YB_REQUIRE((stat_sum == nullptr) == (stat_sqsum == nullptr), YB200_ERR_INVALID, "conv2d_fwd: pass both or neither stat buffer");
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  set_out_view(p, *z);
-  p.epi_mode = stat_sum ? EPI_F16_STATS : EPI_F16;
-  p.stat_sum = stat_sum;
-  p.stat_sq = stat_sqsum;
-  p.stat_fold = stat_fold;
-  return conv_fwd_common(x, w_fwd, z->c, ksize, stride, p, as_stream(stream), 0, 1, stat_fold > 0 ? z->c / stat_fold : 0);
+  return conv2d_fwd_impl("conv2d_fwd_fold", x, w_fwd, z, ksize, stride, stat_sum, stat_sqsum, stat_fold, stream);
 }
 
 extern "C" int yb200_conv2d_bn_silu_fwd(const yb200_act* x, const void* w_fwd, const float* scale, const float* shift,
                                         const yb200_act* residual, const yb200_act* out, int ksize, int stride, void* stream) {
-  int rc;
-  if ((rc = check_act(x, "conv2d_bn_silu_fwd x"))) return rc;
-  if ((rc = check_act(out, "conv2d_bn_silu_fwd out"))) return rc;
-  if (residual && (rc = check_act(residual, "conv2d_bn_silu_fwd residual"))) return rc;
   YB_REQUIRE(scale && shift, YB200_ERR_INVALID, "conv2d_bn_silu_fwd: null scale / shift");
-  YB_REQUIRE(stride == 1 || stride == 2, YB200_ERR_UNSUPPORTED, "conv2d_bn_silu_fwd: stride %d", stride);
-  YB_REQUIRE(out->n == x->n && out->h * stride == x->h && out->w * stride == x->w, YB200_ERR_INVALID,
-             "conv2d_bn_silu_fwd: output %dx%dx%d does not match input %dx%dx%d / stride %d", out->n, out->h, out->w, x->n, x->h, x->w, stride);
-  YB_REQUIRE(!residual || (residual->n == out->n && residual->h == out->h && residual->w == out->w && residual->c == out->c), YB200_ERR_INVALID,
-             "conv2d_bn_silu_fwd: residual shape mismatch");
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  set_out_view(p, *out);
+  int rc;
+  if ((rc = check_fwd("conv2d_bn_silu_fwd", x, out, "out", residual, stride))) return rc;
+  ConvGemmParams p = out_view(*out);
   p.epi_mode = EPI_BF16_BN_SILU;
   p.scale = scale;
   p.shift = shift;
-  if (residual) {
-    p.addend = static_cast<const __nv_bfloat16*>(residual->ptr) + residual->c_off;
-    p.add_sw = residual->c_pitch;
-    p.add_sh = 1LL * residual->c_pitch * residual->w;
-    p.add_sn = 1LL * residual->c_pitch * residual->w * residual->h;
-  }
-  return conv_fwd_common(x, w_fwd, out->c, ksize, stride, p, as_stream(stream));
-}
-
-static void set_addend(ConvGemmParams& p, const yb200_act* a) {
-  p.addend = static_cast<const __nv_bfloat16*>(a->ptr) + a->c_off;
-  p.add_sw = a->c_pitch;
-  p.add_sh = 1LL * a->c_pitch * a->w;
-  p.add_sn = 1LL * a->c_pitch * a->w * a->h;
-}
-static bool same_geometry(const yb200_act* a, const yb200_act* b) {
-  return a->n == b->n && a->h == b->h && a->w == b->w && a->c == b->c && a->c_pitch == b->c_pitch;
+  if (residual) set_addend(p, residual);
+  return conv_fwd_common("conv2d_bn_silu_fwd", x, w_fwd, out->c, out->c, ksize, stride, p, as_stream(stream));
 }
 
 extern "C" int yb200_conv2d_affine_fwd(const yb200_act* x, const void* w_fwd, const float* scale, const float* shift,
                                        const yb200_act* residual, const yb200_act* out, int ksize, int stride, void* stream) {
   int rc;
-  if ((rc = check_act(x, "conv2d_affine_fwd x"))) return rc;
-  if ((rc = check_act(out, "conv2d_affine_fwd out"))) return rc;
-  if (residual && (rc = check_act(residual, "conv2d_affine_fwd residual"))) return rc;
-  YB_REQUIRE(stride == 1 || stride == 2, YB200_ERR_UNSUPPORTED, "conv2d_affine_fwd: stride %d", stride);
-  YB_REQUIRE(out->n == x->n && out->h * stride == x->h && out->w * stride == x->w, YB200_ERR_INVALID,
-             "conv2d_affine_fwd: output %dx%dx%d does not match input %dx%dx%d / stride %d", out->n, out->h, out->w, x->n, x->h, x->w, stride);
-  YB_REQUIRE(!residual || (residual->n == out->n && residual->h == out->h && residual->w == out->w && residual->c == out->c), YB200_ERR_INVALID,
-             "conv2d_affine_fwd: residual shape mismatch");
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  set_out_view(p, *out);
+  if ((rc = check_fwd("conv2d_affine_fwd", x, out, "out", residual, stride))) return rc;
+  ConvGemmParams p = out_view(*out);
   p.epi_mode = EPI_BF16_AFFINE;
   p.scale = scale;
   p.shift = shift;
   if (residual) set_addend(p, residual);
-  return conv_fwd_common(x, w_fwd, out->c, ksize, stride, p, as_stream(stream));
+  return conv_fwd_common("conv2d_affine_fwd", x, w_fwd, out->c, out->c, ksize, stride, p, as_stream(stream));
 }
 
 extern "C" int yb200_conv2d_relu_fwd(const yb200_act* x, const void* w_fwd, const float* bias, const yb200_act* out, int ksize, int stride,
                                      void* stream) {
   int rc;
-  if ((rc = check_act(x, "conv2d_relu_fwd x"))) return rc;
-  if ((rc = check_act(out, "conv2d_relu_fwd out"))) return rc;
-  YB_REQUIRE(stride == 1 || stride == 2, YB200_ERR_UNSUPPORTED, "conv2d_relu_fwd: stride %d", stride);
-  YB_REQUIRE(out->n == x->n && out->h * stride == x->h && out->w * stride == x->w, YB200_ERR_INVALID,
-             "conv2d_relu_fwd: output %dx%dx%d does not match input %dx%dx%d / stride %d", out->n, out->h, out->w, x->n, x->h, x->w, stride);
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  set_out_view(p, *out);
+  if ((rc = check_fwd("conv2d_relu_fwd", x, out, "out", nullptr, stride))) return rc;
+  ConvGemmParams p = out_view(*out);
   p.epi_mode = EPI_BF16_BIAS_RELU;
   p.shift = bias;
-  return conv_fwd_common(x, w_fwd, out->c, ksize, stride, p, as_stream(stream));
+  return conv_fwd_common("conv2d_relu_fwd", x, w_fwd, out->c, out->c, ksize, stride, p, as_stream(stream));
 }
 
 extern "C" int yb200_linear_relu_fwd(const yb200_act* x, const void* w_fwd, const float* bias, const yb200_act* h_out, void* stream) {
   return yb200_conv2d_relu_fwd(x, w_fwd, bias, h_out, 1, 1, stream);
 }
 
-extern "C" int yb200_conv1x1_nchw_f32(const yb200_act* x, const void* w_fwd, const float* bias, int cout, float* out_nchw, void* stream) {
-  int rc;
-  if ((rc = check_act(x, "conv1x1_nchw_f32 x"))) return rc;
-  YB_REQUIRE(out_nchw && cout > 0 && cout <= 128, YB200_ERR_INVALID, "conv1x1_nchw_f32: bad arguments (cout=%d)", cout);
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  const long long hw = 1LL * x->h * x->w;
-  p.out = out_nchw;                 // element (n, y, x, c) at n*cout*hw + c*hw + y*w + x: lanes (pixels) write consecutive floats per channel
-  p.out_sn = 1LL * cout * hw;
-  p.out_sh = x->w;
-  p.out_sw = 1;
-  YB_REQUIRE(hw < (1LL << 31), YB200_ERR_UNSUPPORTED, "conv1x1_nchw_f32: plane too large");
-  p.out_sc = static_cast<int>(hw);
-  p.out_mh = 1; p.out_mw = 1;
-  p.bias = bias;                    // may be null (staged as zeros)
-  p.epi_mode = EPI_F32_BIAS;
-  return conv_fwd_common(x, w_fwd, cout, 1, 1, p, as_stream(stream));
-}
-
-// the same with one weight matrix PER IMAGE (w_fwd: [n][cout][cin] bf16, i.e. n * cout rows): torch.bmm(pred_kernel, mask_features) of a whole batch
-// in one launch.  Pixel tiles must not span images (h * w a multiple of the 128-pixel tile: choose_tile then keeps tiles inside one image).
-extern "C" int yb200_conv1x1_nchw_f32_batched(const yb200_act* x, const void* w_fwd, int cout, float* out_nchw, void* stream) {
-  int rc;
-  if ((rc = check_act(x, "conv1x1_nchw_f32_batched x"))) return rc;
-  YB_REQUIRE(out_nchw && cout > 0 && cout <= 128, YB200_ERR_INVALID, "conv1x1_nchw_f32_batched: bad arguments (cout=%d)", cout);
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  const long long hw = 1LL * x->h * x->w;
-  p.out = out_nchw;
-  p.out_sn = 1LL * cout * hw;
-  p.out_sh = x->w;
-  p.out_sw = 1;
-  YB_REQUIRE(hw < (1LL << 31), YB200_ERR_UNSUPPORTED, "conv1x1_nchw_f32_batched: plane too large");
-  p.out_sc = static_cast<int>(hw);
-  p.out_mh = 1; p.out_mw = 1;
-  p.epi_mode = EPI_F32_BIAS;
-  p.b_img_rows = cout;
-  set_tiles(p, x->n, x->h, x->w);
-  YB_REQUIRE(p.log_tw + p.log_th == 7, YB200_ERR_UNSUPPORTED,
-             "conv1x1_nchw_f32_batched: a 128-pixel tile would span images at %dx%d (use yb200_conv1x1_nchw_f32 per image)", x->h, x->w);
-  // conv_fwd_common, with the weight matrix map covering all images' rows
-  const int bk = pick_block_k(x->c);
-  YB_REQUIRE(bk != 0, YB200_ERR_UNSUPPORTED, "conv1x1_nchw_f32_batched: input channels %d must be a multiple of 16", x->c);
-  const int bn = pick_block_n(cout);
-  p.num_taps = fill_fwd_taps(p.taps, *x, 1, 1, x->c);
-  p.cin_blocks = x->c / bk;
-  p.cout = cout;
-  const int tw = 1 << p.log_tw, th = 1 << p.log_th;
-  CUtensorMap tmA, tmB;
-  if ((rc = make_act_map(&tmA, *x, false, bk, tw, th, 1))) return rc;
-  if ((rc = make_mat_map(&tmB, w_fwd, 1LL * x->n * cout, x->c, bn, bk))) return rc;
-  dim3 grid(p.tiles_w * p.tiles_h * p.tiles_n, ceil_div(cout, bn));
-  return launch_conv(bn, bk, tmA, tmB, p, grid, as_stream(stream));
-}
-
 extern "C" int yb200_linear_gelu_fwd(const yb200_act* x, const void* w_fwd, const float* bias, const yb200_act* u_out, const yb200_act* h_out,
                                      void* stream) {
   int rc;
-  if ((rc = check_act(x, "linear_gelu_fwd x"))) return rc;
-  if ((rc = check_act(h_out, "linear_gelu_fwd h"))) return rc;
+  if ((rc = check_fwd("linear_gelu_fwd", x, h_out, "h", nullptr, 1))) return rc;
   if (u_out && (rc = check_act(u_out, "linear_gelu_fwd u"))) return rc;
-  YB_REQUIRE(h_out->n == x->n && h_out->h == x->h && h_out->w == x->w, YB200_ERR_INVALID, "linear_gelu_fwd: pixel grids differ");
   YB_REQUIRE(!u_out || same_geometry(u_out, h_out), YB200_ERR_INVALID, "linear_gelu_fwd: u and h must have the same shape and channel pitch");
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  set_out_view(p, *h_out);
+  ConvGemmParams p = out_view(*h_out);
   p.epi_mode = EPI_BF16_BIAS_GELU;
   p.shift = bias;
   if (u_out) p.aux_out = static_cast<__nv_bfloat16*>(u_out->ptr) + u_out->c_off;
-  return conv_fwd_common(x, w_fwd, h_out->c, 1, 1, p, as_stream(stream));
+  return conv_fwd_common("linear_gelu_fwd", x, w_fwd, h_out->c, h_out->c, 1, 1, p, as_stream(stream));
+}
+
+// batched: one weight matrix PER IMAGE (w_fwd: [n][cout][cin] bf16, i.e. n * cout rows), torch.bmm(pred_kernel, mask_features) of a whole batch in
+// one launch.  Pixel tiles must not span images (h * w a multiple of the 128-pixel tile: choose_tile then keeps tiles inside one image).
+static int conv1x1_nchw_impl(const char* who, const yb200_act* x, const void* w_fwd, const float* bias, int cout, float* out_nchw, bool batched,
+                             void* stream) {
+  int rc;
+  if ((rc = check_arg(x, who, "x"))) return rc;
+  YB_REQUIRE(out_nchw && cout > 0 && cout <= 128, YB200_ERR_INVALID, "%s: bad arguments (cout=%d)", who, cout);
+  YB_REQUIRE(1LL * x->h * x->w < (1LL << 31), YB200_ERR_UNSUPPORTED, "%s: plane too large", who);
+  ConvGemmParams p = out_nchw_f32(out_nchw, cout, x->h, x->w);
+  p.bias = bias;  // may be null (staged as zeros)
+  p.epi_mode = EPI_F32_BIAS;
+  if (!batched) return conv_fwd_common(who, x, w_fwd, cout, cout, 1, 1, p, as_stream(stream));
+  int log_tw, log_th;
+  choose_tile(x->n, x->h, x->w, 128, &log_tw, &log_th);
+  YB_REQUIRE(log_tw + log_th == 7, YB200_ERR_UNSUPPORTED, "%s: a 128-pixel tile would span images at %dx%d (use yb200_conv1x1_nchw_f32 per image)", who,
+             x->h, x->w);
+  p.b_img_rows = cout;
+  return conv_fwd_common(who, x, w_fwd, 1LL * x->n * cout, cout, 1, 1, p, as_stream(stream));
+}
+
+extern "C" int yb200_conv1x1_nchw_f32(const yb200_act* x, const void* w_fwd, const float* bias, int cout, float* out_nchw, void* stream) {
+  return conv1x1_nchw_impl("conv1x1_nchw_f32", x, w_fwd, bias, cout, out_nchw, false, stream);
+}
+
+extern "C" int yb200_conv1x1_nchw_f32_batched(const yb200_act* x, const void* w_fwd, int cout, float* out_nchw, void* stream) {
+  return conv1x1_nchw_impl("conv1x1_nchw_f32_batched", x, w_fwd, nullptr, cout, out_nchw, true, stream);
+}
+
+// lo_delta = 0, planes = 1: the plain bf16 form; lo_delta > 0: the strict form (conv_fwd_common)
+static int conv1x1_bias_f32_impl(const char* who, const yb200_act* x, int lo_delta, int planes, const void* w_fwd, const float* bias, int cout,
+                                 float* out, int a_total, int a_off, int c_total, int c_off, void* stream) {
+  int rc;
+  if ((rc = check_arg(x, who, "x"))) return rc;
+  YB_REQUIRE(bias && out && cout > 0 && cout <= 128, YB200_ERR_INVALID, "%s: bad arguments (cout=%d)", who, cout);
+  YB_REQUIRE(a_off >= 0 && a_off + x->h * x->w <= a_total && c_off >= 0 && c_off + cout <= c_total, YB200_ERR_INVALID,
+             "%s: slice [%d+%d, %d+%d] outside [%d, %d]", who, a_off, x->h * x->w, c_off, cout, a_total, c_total);
+  ConvGemmParams p = out_rows_f32(out, x->w, a_total, a_off, c_total, c_off);
+  p.bias = bias;
+  p.epi_mode = EPI_F32_BIAS;
+  return conv_fwd_common(who, x, w_fwd, cout, cout, 1, 1, p, as_stream(stream), lo_delta, planes);
 }
 
 extern "C" int yb200_conv1x1_bias_f32(const yb200_act* x, const void* w_fwd, const float* bias, int cout, float* out,
                                       int a_total, int a_off, int c_total, int c_off, void* stream) {
-  int rc;
-  if ((rc = check_act(x, "conv1x1_bias_f32 x"))) return rc;
-  YB_REQUIRE(bias && out && cout > 0 && cout <= 128, YB200_ERR_INVALID, "conv1x1_bias_f32: bad arguments (cout=%d)", cout);
-  YB_REQUIRE(a_off >= 0 && a_off + x->h * x->w <= a_total && c_off >= 0 && c_off + cout <= c_total, YB200_ERR_INVALID,
-             "conv1x1_bias_f32: slice [%d+%d, %d+%d] outside [%d, %d]", a_off, x->h * x->w, c_off, cout, a_total, c_total);
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  p.out = out + 1LL * a_off * c_total + c_off;
-  p.out_sn = 1LL * a_total * c_total;
-  p.out_sh = 1LL * x->w * c_total;
-  p.out_sw = c_total;
-  p.out_sc = 1;
-  p.out_mh = 1; p.out_mw = 1;
-  p.bias = bias;
-  p.epi_mode = EPI_F32_BIAS;
-  return conv_fwd_common(x, w_fwd, cout, 1, 1, p, as_stream(stream));
+  return conv1x1_bias_f32_impl("conv1x1_bias_f32", x, 0, 1, w_fwd, bias, cout, out, a_total, a_off, c_total, c_off, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -551,37 +535,15 @@ extern "C" int yb200_conv2d_fwd_split(const yb200_act* x, int lo_delta, int plan
   YB_REQUIRE(z && cout > 0 && z_off >= 0 && z_off + cout <= z_pitch && lo_delta > 0, YB200_ERR_INVALID,
              "conv2d_fwd_split: bad output slice [%d, %d) of %d (lo_delta %d)", z_off, z_off + cout, z_pitch, lo_delta);
   YB_REQUIRE(stride == 1 || stride == 2, YB200_ERR_UNSUPPORTED, "conv2d_fwd_split: stride %d", stride);
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  const int oh = x->h / stride, ow = x->w / stride;
-  p.out = z + z_off;  // fp32 NHWC with a channel pitch
-  p.out_sw = z_pitch;
-  p.out_sh = 1LL * z_pitch * ow;
-  p.out_sn = 1LL * z_pitch * ow * oh;
-  p.out_sc = 1;
-  p.out_mh = 1; p.out_mw = 1;
+  ConvGemmParams p = out_nhwc_f32(z + z_off, z_pitch, x->h / stride, x->w / stride);
   p.epi_mode = EPI_F32_BIAS;  // bias == null: staged as zeros
-  return conv_fwd_common(x, w_split, cout, ksize, stride, p, as_stream(stream), lo_delta, planes);
+  return conv_fwd_common("conv2d_fwd_split", x, w_split, cout, cout, ksize, stride, p, as_stream(stream), lo_delta, planes);
 }
 
 extern "C" int yb200_conv1x1_bias_f32_split(const yb200_act* x, int lo_delta, int planes, const void* w_split, const float* bias, int cout, float* out,
                                             int a_total, int a_off, int c_total, int c_off, void* stream) {
-  int rc;
-  if ((rc = check_act(x, "conv1x1_bias_f32_split x"))) return rc;
-  YB_REQUIRE(bias && out && cout > 0 && cout <= 128 && lo_delta > 0, YB200_ERR_INVALID, "conv1x1_bias_f32_split: bad arguments (cout=%d)", cout);
-  YB_REQUIRE(a_off >= 0 && a_off + x->h * x->w <= a_total && c_off >= 0 && c_off + cout <= c_total, YB200_ERR_INVALID,
-             "conv1x1_bias_f32_split: slice [%d+%d, %d+%d] outside [%d, %d]", a_off, x->h * x->w, c_off, cout, a_total, c_total);
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  p.out = out + 1LL * a_off * c_total + c_off;
-  p.out_sn = 1LL * a_total * c_total;
-  p.out_sh = 1LL * x->w * c_total;
-  p.out_sw = c_total;
-  p.out_sc = 1;
-  p.out_mh = 1; p.out_mw = 1;
-  p.bias = bias;
-  p.epi_mode = EPI_F32_BIAS;
-  return conv_fwd_common(x, w_split, cout, 1, 1, p, as_stream(stream), lo_delta, planes);
+  YB_REQUIRE(lo_delta > 0, YB200_ERR_INVALID, "conv1x1_bias_f32_split: lo_delta %d", lo_delta);
+  return conv1x1_bias_f32_impl("conv1x1_bias_f32_split", x, lo_delta, planes, w_split, bias, cout, out, a_total, a_off, c_total, c_off, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -607,9 +569,7 @@ static int dgrad_impl(const yb200_act* dz, const void* w_dgrad, const yb200_act*
   const int taps_total = ksize * ksize;
   cudaStream_t st = as_stream(stream);
 
-  ConvGemmParams p;
-  memset(&p, 0, sizeof(p));
-  set_out_view(p, *dx);
+  ConvGemmParams p = out_view(*dx);
   p.epi_mode = EPI_BF16;
   if (gelu_u) {
     p.epi_mode = act_mode;
@@ -618,12 +578,7 @@ static int dgrad_impl(const yb200_act* dz, const void* w_dgrad, const yb200_act*
   }
   p.cout = cin;
   p.cin_blocks = dz->c / bk;
-  if (addend) {
-    p.addend = static_cast<const __nv_bfloat16*>(addend->ptr) + addend->c_off;
-    p.add_sw = addend->c_pitch;
-    p.add_sh = 1LL * addend->c_pitch * addend->w;
-    p.add_sn = 1LL * addend->c_pitch * addend->w * addend->h;
-  }
+  if (addend) set_addend(p, addend);
   set_tiles(p, dz->n, dz->h, dz->w);  // pixel grid = dz grid (for stride 2: each work item is one output-parity class of a tile)
   const int tw = 1 << p.log_tw, th = 1 << p.log_th, tn = 128 >> (p.log_tw + p.log_th);
   CUtensorMap tmA, tmB;
@@ -704,6 +659,7 @@ struct WgradPlan {
   int splits;
   int smem;
   int tw, th, tn;
+  long long workspace_bytes() const { return 4LL * splits * p.cout * p.num_taps * p.cin; }  // fp32 partial sums of every split
 };
 
 int plan_wgrad(const yb200_act* x, const yb200_act* dz, int ksize, int stride, WgradPlan* pl, int group = 0) {
@@ -781,33 +737,30 @@ extern "C" int64_t yb200_conv2d_wgrad_workspace(const yb200_act* x, const yb200_
   WgradPlan pl;
   int rc = plan_wgrad(x, dz, ksize, stride, &pl);
   if (rc) return rc;
-  return 4LL * pl.splits * pl.p.cout * pl.p.num_taps * pl.p.cin;
+  return pl.workspace_bytes();
 }
 
 template <int BN, int TPC>
 static int launch_wgrad_inst(const CUtensorMap& tmDz, const CUtensorMap& tmX, const WgradPlan& pl, dim3 grid, cudaStream_t st) {
-  static PerDevice<int> max_set_dev(0);
-  int& max_set = max_set_dev.cur();
-  if (pl.smem > max_set) {
-    YB_CHECK_CUDA(cudaFuncSetAttribute(wgrad_gemm_kernel<BN, TPC>, cudaFuncAttributeMaxDynamicSharedMemorySize, pl.smem));
-    max_set = pl.smem;
-  }
+  static PerDevice<int> smem_limit(0);
+  YB_CHECK_CUDA(raise_smem_limit(smem_limit, pl.smem, wgrad_gemm_kernel<BN, TPC>));
   launch_k_opt(false, wgrad_gemm_kernel<BN, TPC>, grid, kWgThreads, pl.smem, st, tmDz, tmX, pl.p);
   YB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }
 
-static int wgrad_impl(const yb200_act* x, const yb200_act* dz, int ksize, int stride, int cin_real, int group, float* grad_oihw, int accumulate,
-                      void* workspace, int64_t workspace_bytes, void* stream);
-extern "C" int yb200_conv2d_wgrad(const yb200_act* x, const yb200_act* dz, int ksize, int stride, int cin_real, float* grad_oihw,
-                                  int accumulate, void* workspace, int64_t workspace_bytes, void* stream) {
-  return wgrad_impl(x, dz, ksize, stride, cin_real, 0, grad_oihw, accumulate, workspace, workspace_bytes, stream);
+static int launch_wgrad(const CUtensorMap& tmDz, const CUtensorMap& tmX, const WgradPlan& pl, dim3 grid, cudaStream_t st) {
+  const int bn = pl.p.bn, tpc = pl.p.tpc;
+#define YB_CASE(BN, TPC) \
+  if (bn == BN && tpc == TPC) return launch_wgrad_inst<BN, TPC>(tmDz, tmX, pl, grid, st);
+  YB_CASE(16, 1) YB_CASE(16, 3)
+  YB_CASE(32, 1) YB_CASE(32, 3)
+  YB_CASE(64, 1) YB_CASE(64, 3)
+  YB_CASE(128, 1)
+#undef YB_CASE
+  return fail(YB200_ERR_UNSUPPORTED, "conv2d_wgrad: no kernel for a %d-wide cin tile with %d taps per CTA", bn, tpc);
 }
-extern "C" int yb200_conv2d_wgrad_grouped(const yb200_act* x, const yb200_act* dz, int ksize, int stride, int cin_real, int group, float* grad_oihw,
-                                          int accumulate, void* workspace, int64_t workspace_bytes, void* stream) {
-  YB_REQUIRE(group > 1, YB200_ERR_INVALID, "conv2d_wgrad_grouped: group %d (use yb200_conv2d_wgrad)", group);
-  return wgrad_impl(x, dz, ksize, stride, cin_real, group, grad_oihw, accumulate, workspace, workspace_bytes, stream);
-}
+
 static int wgrad_impl(const yb200_act* x, const yb200_act* dz, int ksize, int stride, int cin_real, int group, float* grad_oihw, int accumulate,
                       void* workspace, int64_t workspace_bytes, void* stream) {
   WgradPlan pl;
@@ -815,28 +768,29 @@ static int wgrad_impl(const yb200_act* x, const yb200_act* dz, int ksize, int st
   if (rc) return rc;
   YB_REQUIRE(grad_oihw && workspace, YB200_ERR_INVALID, "conv2d_wgrad: null pointer");
   YB_REQUIRE(cin_real > 0 && cin_real <= x->c, YB200_ERR_INVALID, "conv2d_wgrad: cin_real %d vs padded %d", cin_real, x->c);
-  const int64_t need = 4LL * pl.splits * pl.p.cout * pl.p.num_taps * pl.p.cin;
-  YB_REQUIRE(workspace_bytes >= need, YB200_ERR_INVALID, "conv2d_wgrad: workspace %lld < %lld bytes", (long long)workspace_bytes,
-             (long long)need);
+  YB_REQUIRE(workspace_bytes >= pl.workspace_bytes(), YB200_ERR_INVALID, "conv2d_wgrad: workspace %lld < %lld bytes", (long long)workspace_bytes,
+             pl.workspace_bytes());
   pl.p.ws = static_cast<float*>(workspace);
   cudaStream_t st = as_stream(stream);
   CUtensorMap tmDz, tmX;
   if ((rc = make_act_map(&tmDz, *dz, false, pl.p.kc_a, pl.tw, pl.th, pl.tn))) return rc;
   if ((rc = make_act_map(&tmX, *x, stride == 2, pl.p.kc_b, pl.tw, pl.th, pl.tn))) return rc;
   dim3 grid(pl.p.cout_tiles * pl.p.cin_tiles * pl.p.tap_groups, pl.splits);
-  const int bn = pl.p.bn, tpc = pl.p.tpc;
-  if (bn == 16 && tpc == 1) rc = launch_wgrad_inst<16, 1>(tmDz, tmX, pl, grid, st);
-  else if (bn == 16 && tpc == 3) rc = launch_wgrad_inst<16, 3>(tmDz, tmX, pl, grid, st);
-  else if (bn == 32 && tpc == 1) rc = launch_wgrad_inst<32, 1>(tmDz, tmX, pl, grid, st);
-  else if (bn == 32 && tpc == 3) rc = launch_wgrad_inst<32, 3>(tmDz, tmX, pl, grid, st);
-  else if (bn == 64 && tpc == 1) rc = launch_wgrad_inst<64, 1>(tmDz, tmX, pl, grid, st);
-  else if (bn == 64 && tpc == 3) rc = launch_wgrad_inst<64, 3>(tmDz, tmX, pl, grid, st);
-  else if (bn == 128 && tpc == 1) rc = launch_wgrad_inst<128, 1>(tmDz, tmX, pl, grid, st);
-  else return fail(YB200_ERR_UNSUPPORTED, "conv2d_wgrad: no kernel for a %d-wide cin tile with %d taps per CTA", bn, tpc);
-  if (rc) return rc;
+  if ((rc = launch_wgrad(tmDz, tmX, pl, grid, st))) return rc;
   const long long total = 1LL * pl.p.cout * pl.p.num_taps * pl.p.cin;
   const int blocks = static_cast<int>(std::min<long long>((total + 31) / 32, 16 * sm_count()));
   launch_k_opt(false, wgrad_reduce_kernel, blocks, 256, 0, st, pl.p.ws, grad_oihw, pl.splits, pl.p.cout, pl.p.num_taps, pl.p.cin, cin_real, accumulate);
   YB_CHECK_CUDA(cudaGetLastError());
   return 0;
+}
+
+extern "C" int yb200_conv2d_wgrad(const yb200_act* x, const yb200_act* dz, int ksize, int stride, int cin_real, float* grad_oihw,
+                                  int accumulate, void* workspace, int64_t workspace_bytes, void* stream) {
+  return wgrad_impl(x, dz, ksize, stride, cin_real, 0, grad_oihw, accumulate, workspace, workspace_bytes, stream);
+}
+
+extern "C" int yb200_conv2d_wgrad_grouped(const yb200_act* x, const yb200_act* dz, int ksize, int stride, int cin_real, int group, float* grad_oihw,
+                                          int accumulate, void* workspace, int64_t workspace_bytes, void* stream) {
+  YB_REQUIRE(group > 1, YB200_ERR_INVALID, "conv2d_wgrad_grouped: group %d (use yb200_conv2d_wgrad)", group);
+  return wgrad_impl(x, dz, ksize, stride, cin_real, group, grad_oihw, accumulate, workspace, workspace_bytes, stream);
 }

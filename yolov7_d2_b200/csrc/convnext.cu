@@ -22,14 +22,6 @@ struct ActV {  // device-side view
 inline ActV viewc(const yb200_act* a) {
   return ActV{static_cast<const __nv_bfloat16*>(a->ptr) + a->c_off, a->n, a->h, a->w, a->c, a->c_pitch};
 }
-int check_view(const yb200_act* a, const char* name, int mult) {
-  YB_REQUIRE(a && a->ptr, YB200_ERR_INVALID, "%s: null view", name);
-  YB_REQUIRE(a->n > 0 && a->h > 0 && a->w > 0 && a->c > 0, YB200_ERR_INVALID, "%s: empty extent", name);
-  YB_REQUIRE(a->c % mult == 0 && a->c_pitch % mult == 0 && a->c_off % mult == 0 && a->c_off + a->c <= a->c_pitch, YB200_ERR_INVALID,
-             "%s: channels (c=%d pitch=%d off=%d) must be multiples of %d with off+c<=pitch", name, a->c, a->c_pitch, a->c_off, mult);
-  return 0;
-}
-bool same_shape(const yb200_act* a, const yb200_act* b) { return a->n == b->n && a->h == b->h && a->w == b->w && a->c == b->c; }
 
 // ------------------------------------------------------------------------------------------------------------------------------
 // depthwise 7x7, stride 1, zero padding 3
@@ -575,9 +567,9 @@ int ln_grid(long long npix) {
 extern "C" int yb200_dwconv7(const yb200_act* x, const float* w_c49, const float* bias, const yb200_act* addend, const yb200_act* out, int flip,
                              void* stream) {
   int rc;
-  if ((rc = check_view(x, "dwconv7 x", 32))) return rc;
-  if ((rc = check_view(out, "dwconv7 out", 32))) return rc;
-  if (addend && (rc = check_view(addend, "dwconv7 addend", 8))) return rc;
+  if ((rc = check_act(x, "dwconv7 x", 32))) return rc;
+  if ((rc = check_act(out, "dwconv7 out", 32))) return rc;
+  if (addend && (rc = check_act(addend, "dwconv7 addend"))) return rc;
   YB_REQUIRE(w_c49 != nullptr, YB200_ERR_INVALID, "dwconv7: null weights");
   YB_REQUIRE(same_shape(x, out) && (!addend || same_shape(addend, out)), YB200_ERR_INVALID, "dwconv7: shapes differ");
   const int tiles_w = ceil_div(x->w, kDwTW), tiles_h = ceil_div(x->h, kDwTH);
@@ -610,20 +602,16 @@ extern "C" int64_t yb200_dwconv7_wgrad_workspace(const yb200_act* x) {
 extern "C" int yb200_dwconv7_wgrad(const yb200_act* x, const yb200_act* dy, float* grad_w_c49, float* grad_bias, int accumulate, void* workspace,
                                    void* stream) {
   int rc;
-  if ((rc = check_view(x, "dwconv7_wgrad x", 32))) return rc;
-  if ((rc = check_view(dy, "dwconv7_wgrad dy", 32))) return rc;
+  if ((rc = check_act(x, "dwconv7_wgrad x", 32))) return rc;
+  if ((rc = check_act(dy, "dwconv7_wgrad dy", 32))) return rc;
   YB_REQUIRE(same_shape(x, dy) && grad_w_c49 && workspace, YB200_ERR_INVALID, "dwconv7_wgrad: bad arguments");
   const int tiles_w = ceil_div(x->w, kDwTW), tiles_h = ceil_div(x->h, kDwTH);
   const int per = dwg_ctas_per_slice(x);
   const int slices = x->c / kDwC;
   cudaStream_t st = as_stream(stream);
   constexpr int kSmem = (kDwHH * kDwRow + kDwTH * kDwTW) * kDwPixWords * 4;
-  static PerDevice<bool> attr_set_dev(false);
-  bool& attr_set = attr_set_dev.cur();
-  if (!attr_set) {
-    YB_CHECK_CUDA(cudaFuncSetAttribute(dwconv7_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-    attr_set = true;
-  }
+  static PerDevice<int> smem_limit(0);
+  YB_CHECK_CUDA(raise_smem_limit(smem_limit, kSmem, dwconv7_wgrad_kernel));
   launch_k(dwconv7_wgrad_kernel, slices * per, kDwgThreads, kSmem, st, viewc(x), viewc(dy), static_cast<float*>(workspace), tiles_w, tiles_h,
                                                              tiles_w * tiles_h * x->n, per);
   launch_k(dwconv7_wgrad_reduce_kernel, ceil_div(x->c * 50, 256), 256, 0, st, static_cast<const float*>(workspace), per, x->c, grad_w_c49, grad_bias, accumulate);
@@ -634,8 +622,8 @@ extern "C" int yb200_dwconv7_wgrad(const yb200_act* x, const yb200_act* dy, floa
 extern "C" int yb200_layernorm_fwd(const yb200_act* x, const float* gamma, const float* beta, float eps, const yb200_act* y, float* stats_mean_rstd,
                                    void* stream) {
   int rc;
-  if ((rc = check_view(x, "layernorm_fwd x", 4))) return rc;
-  if ((rc = check_view(y, "layernorm_fwd y", 4))) return rc;
+  if ((rc = check_act(x, "layernorm_fwd x", 4))) return rc;
+  if ((rc = check_act(y, "layernorm_fwd y", 4))) return rc;
   YB_REQUIRE(gamma && beta && same_shape(x, y), YB200_ERR_INVALID, "layernorm_fwd: bad arguments");
   const long long npix = 1LL * x->n * x->h * x->w;
   cudaStream_t st = as_stream(stream);
@@ -658,10 +646,10 @@ extern "C" int64_t yb200_layernorm_bwd_workspace(const yb200_act* x) {
 extern "C" int yb200_layernorm_bwd(const yb200_act* dy, const yb200_act* x, const float* stats_mean_rstd, const float* gamma, const yb200_act* addend,
                                    const yb200_act* dx, float* grad_gamma, float* grad_beta, int accumulate, void* workspace, void* stream) {
   int rc;
-  if ((rc = check_view(dy, "layernorm_bwd dy", 4))) return rc;
-  if ((rc = check_view(x, "layernorm_bwd x", 4))) return rc;
-  if ((rc = check_view(dx, "layernorm_bwd dx", 4))) return rc;
-  if (addend && (rc = check_view(addend, "layernorm_bwd addend", 4))) return rc;
+  if ((rc = check_act(dy, "layernorm_bwd dy", 4))) return rc;
+  if ((rc = check_act(x, "layernorm_bwd x", 4))) return rc;
+  if ((rc = check_act(dx, "layernorm_bwd dx", 4))) return rc;
+  if (addend && (rc = check_act(addend, "layernorm_bwd addend", 4))) return rc;
   YB_REQUIRE(stats_mean_rstd && gamma && grad_gamma && grad_beta && workspace, YB200_ERR_INVALID, "layernorm_bwd: null pointer");
   YB_REQUIRE(same_shape(dy, x) && same_shape(dx, x) && (!addend || same_shape(addend, x)), YB200_ERR_INVALID, "layernorm_bwd: shapes differ");
   const long long npix = 1LL * x->n * x->h * x->w;
@@ -672,13 +660,9 @@ extern "C" int yb200_layernorm_bwd(const yb200_act* dy, const yb200_act* x, cons
   __nv_bfloat16* dxp = static_cast<__nv_bfloat16*>(dx->ptr) + dx->c_off;
   rc = dispatch_steps(x->c, [&](auto steps) {
     constexpr int S = decltype(steps)::value;
-    static PerDevice<bool> attr_set_dev(false);
-  bool& attr_set = attr_set_dev.cur();  // per instantiation
-    if (!attr_set) {
-      cudaError_t e = cudaFuncSetAttribute(layernorm_bwd_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLnWarps * 2 * S * 128 * 4);
-      if (e != cudaSuccess) return fail(YB200_ERR_CUDA, "layernorm_bwd: %s", cudaGetErrorString(e));
-      attr_set = true;
-    }
+    static PerDevice<int> smem_limit(0);  // per instantiation
+    const cudaError_t e = raise_smem_limit(smem_limit, kLnWarps * 2 * S * 128 * 4, layernorm_bwd_kernel<S>);
+    if (e != cudaSuccess) return fail(YB200_ERR_CUDA, "layernorm_bwd: %s", cudaGetErrorString(e));
     launch_k(layernorm_bwd_kernel<S>, blocks, kLnWarps * 32, smem, st, viewc(dy), viewc(x), reinterpret_cast<const float2*>(stats_mean_rstd), gamma, av, dxp,
                                                                  dx->c_pitch, static_cast<float*>(workspace), npix);
     return 0;
@@ -697,7 +681,7 @@ extern "C" int64_t yb200_colsum_workspace(const yb200_act* x) {
 
 extern "C" int yb200_colsum(const yb200_act* x, float scale, float* out, int accumulate, void* workspace, void* stream) {
   int rc;
-  if ((rc = check_view(x, "colsum x", 8))) return rc;
+  if ((rc = check_act(x, "colsum x"))) return rc;
   YB_REQUIRE(out && workspace, YB200_ERR_INVALID, "colsum: null pointer");
   YB_REQUIRE(x->c / 8 <= 256, YB200_ERR_UNSUPPORTED, "colsum: %d channels (max 2048)", x->c);
   const long long npix = 1LL * x->n * x->h * x->w;
@@ -722,7 +706,7 @@ extern "C" int yb200_layer_scale_grad(const float* raw_wgrad, const float* w2, c
 
 extern "C" int yb200_patchify4(const void* images_nchw, int is_f32, int n, int h, int w, const yb200_act* out, void* stream) {
   int rc;
-  if ((rc = check_view(out, "patchify4 out", 8))) return rc;
+  if ((rc = check_act(out, "patchify4 out"))) return rc;
   YB_REQUIRE(images_nchw && n > 0 && h % 4 == 0 && w % 4 == 0, YB200_ERR_INVALID, "patchify4: image %dx%dx%d (H, W must be multiples of 4)", n, h, w);
   YB_REQUIRE(out->n == n && out->h == h / 4 && out->w == w / 4 && out->c == 48, YB200_ERR_INVALID, "patchify4: output must be [%d][%d][%d][48]", n, h / 4,
              w / 4);
@@ -747,9 +731,9 @@ extern "C" int yb200_f64_to_f32(double* src, int n, float* dst, int accumulate, 
 
 extern "C" int yb200_add(const yb200_act* a, const yb200_act* b, const yb200_act* out, void* stream) {
   int rc;
-  if ((rc = check_view(a, "add a", 8))) return rc;
-  if ((rc = check_view(b, "add b", 8))) return rc;
-  if ((rc = check_view(out, "add out", 8))) return rc;
+  if ((rc = check_act(a, "add a"))) return rc;
+  if ((rc = check_act(b, "add b"))) return rc;
+  if ((rc = check_act(out, "add out"))) return rc;
   YB_REQUIRE(same_shape(a, b) && same_shape(a, out), YB200_ERR_INVALID, "add: shapes differ");
   const long long npix = 1LL * a->n * a->h * a->w;
   const long long total = npix * (a->c / 8);
@@ -761,8 +745,8 @@ extern "C" int yb200_add(const yb200_act* a, const yb200_act* b, const yb200_act
 
 extern "C" int yb200_sigmoid(const yb200_act* x, const yb200_act* out, void* stream) {
   int rc;
-  if ((rc = check_view(x, "sigmoid x", 8))) return rc;
-  if ((rc = check_view(out, "sigmoid out", 8))) return rc;
+  if ((rc = check_act(x, "sigmoid x"))) return rc;
+  if ((rc = check_act(out, "sigmoid out"))) return rc;
   YB_REQUIRE(same_shape(x, out), YB200_ERR_INVALID, "sigmoid: shapes differ");
   const long long npix = 1LL * x->n * x->h * x->w;
   const long long total = npix * (x->c / 8);
@@ -774,7 +758,7 @@ extern "C" int yb200_sigmoid(const yb200_act* x, const yb200_act* out, void* str
 
 extern "C" int yb200_iam_normalize(const float* raw, const float* normalizer, int rows, int cols, const yb200_act* out, void* stream) {
   int rc;
-  if ((rc = check_view(out, "iam_normalize out", 8))) return rc;
+  if ((rc = check_act(out, "iam_normalize out"))) return rc;
   YB_REQUIRE(raw && normalizer && rows > 0 && cols > 0, YB200_ERR_INVALID, "iam_normalize: bad arguments");
   YB_REQUIRE(out->n == 1 && out->h == 1 && out->w == rows && out->c == cols, YB200_ERR_INVALID, "iam_normalize: output must be a [1][1][%d][%d] view", rows, cols);
   launch_k(iam_normalize_kernel, ceil_div(rows * cols, 256), 256, 0, as_stream(stream), raw, normalizer, rows, cols, static_cast<__nv_bfloat16*>(out->ptr) + out->c_off,

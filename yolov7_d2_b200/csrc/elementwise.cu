@@ -24,16 +24,6 @@ View mk(const yb200_act* a) {
   return v;
 }
 
-int check_view(const yb200_act* a, const char* name) {
-  YB_REQUIRE(a && a->ptr, YB200_ERR_INVALID, "%s: null view", name);
-  YB_REQUIRE(a->n > 0 && a->h > 0 && a->w > 0 && a->c > 0 && a->c % 8 == 0 && a->c_pitch % 8 == 0 && a->c_off % 8 == 0 &&
-                 a->c_off + a->c <= a->c_pitch,
-             YB200_ERR_INVALID, "%s: bad view n=%d h=%d w=%d c=%d pitch=%d off=%d", name, a->n, a->h, a->w, a->c, a->c_pitch, a->c_off);
-  return 0;
-}
-
-bool same_shape(const yb200_act* a, const yb200_act* b) { return a->n == b->n && a->h == b->h && a->w == b->w && a->c == b->c; }
-
 // streaming 16-byte load (read once: do not allocate in L1)
 // YB200_L2_ORDER=1: element-wise passes walk their tensors in the direction that meets the producer's most recent (L2-resident) output first
 static int l2_order() {
@@ -742,9 +732,9 @@ extern "C" int yb200_bn_eval_affine(int c, const float* gamma, const float* beta
 static int bn_apply_impl(const yb200_act* z, const float* scale, const float* shift, const yb200_act* residual, const yb200_act* out,
                          const yb200_act* out_up2x, const BnFinalize& fin, void* stream) {
   int rc;
-  if ((rc = check_view(z, "bn_apply_silu z")) || (rc = check_view(out, "bn_apply_silu out"))) return rc;
-  if (residual && (rc = check_view(residual, "bn_apply_silu residual"))) return rc;
-  if (out_up2x && (rc = check_view(out_up2x, "bn_apply_silu out_up2x"))) return rc;
+  if ((rc = check_act(z, "bn_apply_silu z")) || (rc = check_act(out, "bn_apply_silu out"))) return rc;
+  if (residual && (rc = check_act(residual, "bn_apply_silu residual"))) return rc;
+  if (out_up2x && (rc = check_act(out_up2x, "bn_apply_silu out_up2x"))) return rc;
   YB_REQUIRE((scale && shift) || fin.ssum, YB200_ERR_INVALID, "bn_apply_silu: null scale/shift");
   YB_REQUIRE(same_shape(z, out) && (!residual || same_shape(z, residual)), YB200_ERR_INVALID, "bn_apply_silu: shape mismatch");
   YB_REQUIRE(!out_up2x || (out_up2x->n == z->n && out_up2x->h == 2 * z->h && out_up2x->w == 2 * z->w && out_up2x->c == z->c), YB200_ERR_INVALID,
@@ -787,9 +777,9 @@ extern "C" int yb200_bn_silu_bwd(const yb200_act* z, const yb200_act* da, const 
                                  const float* shift, const float* save_mean, const float* save_invstd, double* acc_dgamma, double* acc_dbeta,
                                  const yb200_act* dz, float* dgamma, float* dbeta, int accumulate, void* stream) {
   int rc;
-  if ((rc = check_view(z, "bn_silu_bwd z")) || (rc = check_view(da, "bn_silu_bwd da")) || (rc = check_view(dz, "bn_silu_bwd dz"))) return rc;
-  if (da2 && (rc = check_view(da2, "bn_silu_bwd da2"))) return rc;
-  if (da_up2x && (rc = check_view(da_up2x, "bn_silu_bwd da_up2x"))) return rc;
+  if ((rc = check_act(z, "bn_silu_bwd z")) || (rc = check_act(da, "bn_silu_bwd da")) || (rc = check_act(dz, "bn_silu_bwd dz"))) return rc;
+  if (da2 && (rc = check_act(da2, "bn_silu_bwd da2"))) return rc;
+  if (da_up2x && (rc = check_act(da_up2x, "bn_silu_bwd da_up2x"))) return rc;
   YB_REQUIRE(scale && shift && save_mean && save_invstd && acc_dgamma && acc_dbeta && (dgamma != nullptr) == (dbeta != nullptr), YB200_ERR_INVALID,
              "bn_silu_bwd: null pointer");
   YB_REQUIRE(same_shape(z, da) && same_shape(z, dz) && (!da2 || same_shape(z, da2)), YB200_ERR_INVALID, "bn_silu_bwd: shape mismatch");
@@ -814,17 +804,14 @@ extern "C" int yb200_bn_silu_bwd(const yb200_act* z, const yb200_act* da, const 
   const int red_rows = red_shuffle ? static_cast<int>(block.x * block.y) / 32 : static_cast<int>(block.y);
   const size_t red_smem = static_cast<size_t>(red_rows) * 2 * z->c * sizeof(float);
   const unsigned grid_r = static_cast<unsigned>((npix + block.y * red_iters - 1) / (block.y * red_iters));
-  if (src.has_b || src.has_up) {  // fan-out / upsampled gradient sources: the general kernel
-    if (red_smem > 48 * 1024)
-      YB_CHECK_CUDA(cudaFuncSetAttribute(bn_silu_bwd_reduce_kernel<2, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(red_smem)));
+  static PerDevice<int> red_limit(48 * 1024);
+  YB_CHECK_CUDA(raise_smem_limit(red_limit, static_cast<int>(red_smem), bn_silu_bwd_reduce_kernel<2, 3, false>, bn_silu_bwd_reduce_kernel<2, 3, true>));
+  if (src.has_b || src.has_up)  // fan-out / upsampled gradient sources: the general kernel
     launch_k(bn_silu_bwd_reduce_kernel<2, 3, false>, grid_r, block, red_smem, st, vz, src, scale, shift, save_mean, save_invstd, acc_dgamma, acc_dbeta,
                                                                              static_cast<unsigned>(npix), red_iters, l2_order());
-  } else {
-    if (red_smem > 48 * 1024)
-      YB_CHECK_CUDA(cudaFuncSetAttribute(bn_silu_bwd_reduce_kernel<2, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(red_smem)));
+  else
     launch_k(bn_silu_bwd_reduce_kernel<2, 3, true>, grid_r, block, red_smem, st, vz, src, scale, shift, save_mean, save_invstd, acc_dgamma, acc_dbeta,
                                                                             static_cast<unsigned>(npix), red_iters, l2_order());
-  }
   YB_CHECK_CUDA(cudaGetLastError());
   const unsigned grid_a = static_cast<unsigned>((npix + block.y * kEwIters - 1) / (block.y * kEwIters));
   if (!src.has_b && !src.has_up)
@@ -865,19 +852,15 @@ extern "C" int yb200_bn_param_grads(double* acc_dgamma, double* acc_dbeta, int c
 
 extern "C" int yb200_spp_pool(const yb200_act* x, const yb200_act* o5, const yb200_act* o9, const yb200_act* o13, uint8_t* argmax, void* stream) {
   int rc;
-  if ((rc = check_view(x, "spp_pool x")) || (rc = check_view(o5, "spp_pool o5")) || (rc = check_view(o9, "spp_pool o9")) ||
-      (rc = check_view(o13, "spp_pool o13")))
+  if ((rc = check_act(x, "spp_pool x")) || (rc = check_act(o5, "spp_pool o5")) || (rc = check_act(o9, "spp_pool o9")) ||
+      (rc = check_act(o13, "spp_pool o13")))
     return rc;
   YB_REQUIRE(same_shape(x, o5) && same_shape(x, o9) && same_shape(x, o13), YB200_ERR_INVALID, "spp_pool: shape mismatch");
   constexpr int kCg = 16;
   const size_t tiled_smem = static_cast<size_t>(x->h) * x->w * kCg * 2 * sizeof(uint32_t);
   if (x->c % kCg == 0 && tiled_smem <= 200 * 1024) {
-    static PerDevice<size_t> smem_set_dev(48 * 1024);
-    size_t& smem_set = smem_set_dev.cur();
-    if (tiled_smem > smem_set) {
-      YB_CHECK_CUDA(cudaFuncSetAttribute(spp_pool_tiled_kernel<kCg>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tiled_smem)));
-      smem_set = tiled_smem;
-    }
+    static PerDevice<int> smem_limit(48 * 1024);
+    YB_CHECK_CUDA(raise_smem_limit(smem_limit, static_cast<int>(tiled_smem), spp_pool_tiled_kernel<kCg>));
     launch_k(spp_pool_tiled_kernel<kCg>, dim3(x->c / kCg, x->n), 256, tiled_smem, as_stream(stream), mk(x), mk(o5), mk(o9), mk(o13), argmax);
     YB_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -891,8 +874,8 @@ extern "C" int yb200_spp_pool(const yb200_act* x, const yb200_act* o5, const yb2
 extern "C" int yb200_spp_pool_bwd(const yb200_act* d0, const yb200_act* d5, const yb200_act* d9, const yb200_act* d13, const uint8_t* argmax,
                                   float* scratch, const yb200_act* dx, void* stream) {
   int rc;
-  if ((rc = check_view(d0, "spp_pool_bwd d0")) || (rc = check_view(d5, "spp_pool_bwd d5")) || (rc = check_view(d9, "spp_pool_bwd d9")) ||
-      (rc = check_view(d13, "spp_pool_bwd d13")) || (rc = check_view(dx, "spp_pool_bwd dx")))
+  if ((rc = check_act(d0, "spp_pool_bwd d0")) || (rc = check_act(d5, "spp_pool_bwd d5")) || (rc = check_act(d9, "spp_pool_bwd d9")) ||
+      (rc = check_act(d13, "spp_pool_bwd d13")) || (rc = check_act(dx, "spp_pool_bwd dx")))
     return rc;
   YB_REQUIRE(argmax && scratch, YB200_ERR_INVALID, "spp_pool_bwd: null pointer");
   YB_REQUIRE(same_shape(dx, d0) && same_shape(dx, d5) && same_shape(dx, d9) && same_shape(dx, d13), YB200_ERR_INVALID, "spp_pool_bwd: shape mismatch");
@@ -902,12 +885,8 @@ extern "C" int yb200_spp_pool_bwd(const yb200_act* d0, const yb200_act* d5, cons
   // fp32 gradient plane + one branch's bf16 gradients and argmax codes
   const size_t tiled_smem = static_cast<size_t>(dx->h) * dx->w * kCg * (sizeof(float) + sizeof(__nv_bfloat16) + 1);
   if (dx->c % kCg == 0 && tiled_smem <= 200 * 1024) {  // every map the forward pools in shared memory (8 B per element) fits here
-    static PerDevice<size_t> smem_set_dev(48 * 1024);
-    size_t& smem_set = smem_set_dev.cur();
-    if (tiled_smem > smem_set) {
-      YB_CHECK_CUDA(cudaFuncSetAttribute(spp_pool_bwd_tiled_kernel<kCg>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tiled_smem)));
-      smem_set = tiled_smem;
-    }
+    static PerDevice<int> smem_limit(48 * 1024);
+    YB_CHECK_CUDA(raise_smem_limit(smem_limit, static_cast<int>(tiled_smem), spp_pool_bwd_tiled_kernel<kCg>));
     launch_k(spp_pool_bwd_tiled_kernel<kCg>, dim3(dx->c / kCg, dx->n), 256, tiled_smem, st, mk(d0), mk(d5), mk(d9), mk(d13), argmax, mk(dx));
     YB_CHECK_CUDA(cudaGetLastError());
     return 0;
@@ -922,7 +901,7 @@ extern "C" int yb200_spp_pool_bwd(const yb200_act* d0, const yb200_act* d5, cons
 
 extern "C" int yb200_copy_view(const yb200_act* src, const yb200_act* dst, void* stream) {
   int rc;
-  if ((rc = check_view(src, "copy_view src")) || (rc = check_view(dst, "copy_view dst"))) return rc;
+  if ((rc = check_act(src, "copy_view src")) || (rc = check_act(dst, "copy_view dst"))) return rc;
   YB_REQUIRE(same_shape(src, dst), YB200_ERR_INVALID, "copy_view: shape mismatch");
   const long long total = 1LL * src->n * src->h * src->w * (src->c / 8);
   launch_k(copy_view_kernel, grid_for(total, 256), 256, 0, as_stream(stream), mk(src), mk(dst));

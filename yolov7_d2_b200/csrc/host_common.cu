@@ -31,6 +31,14 @@ int sm_count() {
   return n[dev];
 }
 
+int check_act(const yb200_act* a, const char* name, int mult) {
+  YB_REQUIRE(a != nullptr && a->ptr != nullptr, YB200_ERR_INVALID, "%s: null view", name);
+  YB_REQUIRE(a->n > 0 && a->h > 0 && a->w > 0 && a->c > 0, YB200_ERR_INVALID, "%s: empty extent (%dx%dx%dx%d)", name, a->n, a->h, a->w, a->c);
+  YB_REQUIRE(a->c % mult == 0 && a->c_pitch % mult == 0 && a->c_off % mult == 0 && a->c_off + a->c <= a->c_pitch, YB200_ERR_INVALID,
+             "%s: channels (c=%d pitch=%d off=%d) must be multiples of %d with off+c<=pitch", name, a->c, a->c_pitch, a->c_off, mult);
+  return 0;
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);

@@ -31,6 +31,18 @@ struct PerDevice {
   }
 };
 
+// Kernels that take more dynamic shared memory than the default must opt in with a function attribute.  Raises the limit of every kernel
+// in `kernels` to `bytes` when that exceeds what `limit` records for the current device; `limit` is the call site's static cache.
+template <typename... K>
+inline cudaError_t raise_smem_limit(PerDevice<int>& limit, int bytes, K*... kernels) {
+  int& cur = limit.cur();
+  if (bytes <= cur) return cudaSuccess;
+  cudaError_t e = cudaSuccess;
+  ((e = e == cudaSuccess ? cudaFuncSetAttribute(kernels, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) : e), ...);
+  if (e == cudaSuccess) cur = bytes;
+  return e;
+}
+
 #define YB_CHECK_CUDA(expr)                                                                      \
   do {                                                                                           \
     cudaError_t _e = (expr);                                                                     \
@@ -42,6 +54,12 @@ struct PerDevice {
   } while (0)
 
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
+
+// Argument checks of an activation view: non-null, positive extents, and c, c_pitch, c_off multiples of `mult` with c_off + c <= c_pitch.
+// Returns 0 or YB200_ERR_INVALID with a message that starts with `name` (entry point and argument).
+int check_act(const yb200_act* a, const char* name, int mult = 8);
+inline bool same_shape(const yb200_act* a, const yb200_act* b) { return a->n == b->n && a->h == b->h && a->w == b->w && a->c == b->c; }
+inline bool same_geometry(const yb200_act* a, const yb200_act* b) { return same_shape(a, b) && a->c_pitch == b->c_pitch; }
 
 // 5-D TMA view (c, w, p, h, n) of an NHWC bf16 activation.  space_to_depth=false: p is a dummy dimension of
 // extent 1.  space_to_depth=true (stride-2 taps): rows split into (h/2, p=row parity) and the column parity is

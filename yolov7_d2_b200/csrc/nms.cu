@@ -194,7 +194,8 @@ extern "C" int yb200_postprocess_nms_indexed(float* prediction, int batch, int n
   launch_k(nms_prepare_kernel, dim3(ceil_div(apad, 256), batch), 256, 0, st, prediction, num_anchors, 5 + num_classes, apad, conf_thre, mutate_prediction,
                                                                       boxes, meta, keys);
   YB_CHECK_CUDA(cudaGetLastError());
-  YB_CHECK_CUDA(cudaFuncSetAttribute(nms_suppress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));  // per device, cheap
+  static PerDevice<int> smem_limit(0);
+  YB_CHECK_CUDA(raise_smem_limit(smem_limit, static_cast<int>(smem), nms_suppress_kernel));
   launch_k(nms_suppress_kernel, batch, kNmsThreads, smem, st, keys, boxes, meta, num_anchors, num_classes, apad, nms_thre, detections, det_count,
                                                         det_anchor, tie_count);
   YB_CHECK_CUDA(cudaGetLastError());

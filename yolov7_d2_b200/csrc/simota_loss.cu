@@ -656,12 +656,8 @@ extern "C" int yb200_simota_assign(const float* outputs, const float* labels, in
   launch_k(simota_count_gt_kernel, ceil_div(batch, 64), 64, 0, st, labels, batch, max_gt, num_gt, totals);
   YB_CHECK_CUDA(cudaGetLastError());
   const size_t tile = static_cast<size_t>(kPrepAnchors) * channels * sizeof(float);
-  static PerDevice<size_t> prep_smem_dev(0);
-  size_t& prep_smem = prep_smem_dev.cur();
-  if (tile > prep_smem) {
-    YB_CHECK_CUDA(cudaFuncSetAttribute(simota_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tile)));
-    prep_smem = tile;
-  }
+  static PerDevice<int> smem_limit(0);
+  YB_CHECK_CUDA(raise_smem_limit(smem_limit, static_cast<int>(tile), simota_prep_kernel));
   launch_k(simota_prep_kernel, dim3(ceil_div(num_anchors, kPrepAnchors), batch), kPrepAnchors, tile, st, outputs, labels, num_gt, num_anchors, channels,
                                                                                                   max_gt, L, cand, s_all, match_count, totals);
   YB_CHECK_CUDA(cudaGetLastError());
@@ -724,12 +720,8 @@ static int yolox_loss_impl(const float* outputs, const float* labels, int batch,
   out.bias_acc = want_grad ? bias_acc : nullptr;
   cudaStream_t st = as_stream(stream);
   const size_t tile = static_cast<size_t>(kLossAnchors) * channels * sizeof(float);
-  static PerDevice<size_t> loss_smem_dev(0);
-  size_t& loss_smem = loss_smem_dev.cur();
-  if (tile > loss_smem) {
-    YB_CHECK_CUDA(cudaFuncSetAttribute(yolox_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(tile)));
-    loss_smem = tile;
-  }
+  static PerDevice<int> smem_limit(0);
+  YB_CHECK_CUDA(raise_smem_limit(smem_limit, static_cast<int>(tile), yolox_loss_kernel));
   static_assert(kLossAnchors == 128, "Levels::blk_off assumes 128-anchor blocks");
   launch_k(yolox_loss_kernel, dim3(L.blk_off[kMaxLevels], batch), kLossAnchors, tile, st, 
       outputs, labels, num_anchors, channels, max_gt, L, fg_mask, matched_gt, matched_iou, matched_cls, totals, weights3, out, want_loss, want_grad);

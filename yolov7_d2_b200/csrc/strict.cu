@@ -21,7 +21,7 @@ struct SplitView {  // device-side view of a split activation: plane j at p + j 
 };
 
 int mk_split(const yb200_act* a, int lo_delta, int planes, const char* name, SplitView* v) {
-  YB_REQUIRE(a && a->ptr && a->n > 0 && a->h > 0 && a->w > 0 && a->c > 0, YB200_ERR_INVALID, "%s: null / empty view", name);
+  if (const int rc = check_act(a, name, 1)) return rc;
   YB_REQUIRE((planes == 2 || planes == 3) && lo_delta > 0 && a->c_off + (planes - 1) * lo_delta + a->c <= a->c_pitch, YB200_ERR_INVALID,
              "%s: plane %d [%d, %d) outside the pitch %d", name, planes - 1, a->c_off + (planes - 1) * lo_delta,
              a->c_off + (planes - 1) * lo_delta + a->c, a->c_pitch);

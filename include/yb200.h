@@ -409,6 +409,27 @@ typedef struct yb200_mosaic_desc {
 int yb200_mosaic_warp(const yb200_mosaic_desc* table_dev, int n, const uint8_t* src, uint8_t* out, int max_h, int max_w, void* stream);
 int yb200_mosaic_mixup(const yb200_mosaic_desc* table_dev, int n, const uint8_t* src, uint8_t* out, int max_h, int max_w, void* stream);
 
+/* ---- DETR matching cost and SetCriterion (yolov7/utils/detr_utils.py:12-91, yolov7/modeling/meta_arch/detr.py:475-647) ----------------------
+ * Every call covers all L decoder layers.  logits: fp32 [L][B][Q][K1] (K1 = num_classes + 1, the last class is "no object"), boxes: fp32
+ * [L][B][Q][4] post-sigmoid (cx, cy, w, h).  The targets of the batch are packed: labels int32 [G], target_boxes fp32 [G][4] (cx, cy, w, h),
+ * offsets int32 [B+1] (image b owns targets [offsets[b], offsets[b+1]), offsets[B] = G).  labels / target_boxes must not be NULL even when G = 0.
+ *   yb200_detr_match_cost: HungarianMatcher's cost w_bbox * L1 + w_class * (-softmax[label]) + w_giou * (-GIoU) (detr_utils.py:65-86), only the
+ *     per-image blocks: block (l, b) is [Q][G_b] row-major at cost + l*Q*G + Q*offsets[b].  cost has L*Q*G + 1 floats: the last one is an int32
+ *     status word, bit 0 = a label outside [0, K1), bit 1 = a target box whose corners are out of order (generalized_box_iou's assert).
+ *   yb200_detr_set_loss: match int32 [L][B][Q] = the matched target's index within its image, or -1.  out fp32 [L][5] = (loss_ce, loss_bbox,
+ *     loss_giou, cardinality_error, class_error) of each layer, unweighted, as loss_labels / loss_boxes / loss_cardinality (detr.py:507-570)
+ *     compute them; the cross entropy is weighted by eos_coef on the no-object class and normalised by its weight sum; num_boxes as detr.py:620-624.
+ *   yb200_detr_set_loss_bwd: grad fp32 [L][3] = upstream gradients of (loss_ce, loss_bbox, loss_giou) per layer (device memory); writes
+ *     dlogits [L][B][Q][K1] and dboxes [L][B][Q][4] (zero on unmatched queries).
+ * Fixed summation order (bit-reproducible), no host synchronisation.                                                                            */
+int yb200_detr_match_cost(const float* logits, const float* boxes, const int32_t* labels, const float* target_boxes, const int32_t* offsets, int L,
+                          int B, int Q, int K1, int G, float w_class, float w_bbox, float w_giou, float* cost, void* stream);
+int yb200_detr_set_loss(const float* logits, const float* boxes, const int32_t* match, const int32_t* labels, const float* target_boxes,
+                        const int32_t* offsets, int L, int B, int Q, int K1, float eos_coef, float num_boxes, float* out, void* stream);
+int yb200_detr_set_loss_bwd(const float* logits, const float* boxes, const int32_t* match, const int32_t* labels, const float* target_boxes,
+                            const int32_t* offsets, int L, int B, int Q, int K1, float eos_coef, float num_boxes, const float* grad, float* dlogits,
+                            float* dboxes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -114,3 +114,35 @@ def act(t, c_off=0, c=None):
     assert t.dtype in (torch.bfloat16, torch.float16) and t.dim() == 4 and t.is_contiguous(), (t.dtype, t.shape, t.stride())
     n, h, w, cp = t.shape
     return Act(t.data_ptr(), n, h, w, cp - c_off if c is None else c, cp, c_off)
+
+
+def _f32(t):
+    assert t.dtype == torch.float32 and t.is_contiguous(), (t.dtype, t.shape)
+    return ptr(t)
+
+
+def _i32(t):
+    assert t.dtype == torch.int32 and t.is_contiguous(), (t.dtype, t.shape)
+    return ptr(t)
+
+
+def detr_match_cost(logits, boxes, labels, target_boxes, offsets, num_targets, w_class, w_bbox, w_giou, cost):
+    """yb200_detr_match_cost on the current stream: logits [L, B, Q, K1], boxes [L, B, Q, 4] -> cost (L*Q*G floats + the status word)"""
+    L, B, Q, K1 = logits.shape
+    check(lib().yb200_detr_match_cost(_f32(logits), _f32(boxes), _i32(labels), _f32(target_boxes), _i32(offsets), L, B, Q, K1, num_targets,
+                                      c_float(w_class), c_float(w_bbox), c_float(w_giou), _f32(cost), stream_ptr()), "detr_match_cost")
+
+
+def detr_set_loss(logits, boxes, match, labels, target_boxes, offsets, eos_coef, num_boxes, out):
+    """yb200_detr_set_loss on the current stream: out [L, 5] = (loss_ce, loss_bbox, loss_giou, cardinality_error, class_error) per layer"""
+    L, B, Q, K1 = logits.shape
+    check(lib().yb200_detr_set_loss(_f32(logits), _f32(boxes), _i32(match), _i32(labels), _f32(target_boxes), _i32(offsets), L, B, Q, K1,
+                                    c_float(eos_coef), c_float(num_boxes), _f32(out), stream_ptr()), "detr_set_loss")
+
+
+def detr_set_loss_bwd(logits, boxes, match, labels, target_boxes, offsets, eos_coef, num_boxes, grad, dlogits, dboxes):
+    """yb200_detr_set_loss_bwd on the current stream: grad [L, 3] (device) -> dlogits, dboxes shaped like logits, boxes"""
+    L, B, Q, K1 = logits.shape
+    check(lib().yb200_detr_set_loss_bwd(_f32(logits), _f32(boxes), _i32(match), _i32(labels), _f32(target_boxes), _i32(offsets), L, B, Q, K1,
+                                        c_float(eos_coef), c_float(num_boxes), _f32(grad), _f32(dlogits), _f32(dboxes), stream_ptr()),
+          "detr_set_loss_bwd")

@@ -19,6 +19,7 @@ reference's DETR) and `normalize_before=True` are not supported.  There is no CP
 """
 import ctypes
 import os
+import types
 
 import torch
 import torch.nn as nn
@@ -684,3 +685,127 @@ class Transformer(nn.Module):
         memory = self.encoder(src, src_key_padding_mask=mask, pos=pos_embed)
         hs = self.decoder(tgt, memory, memory_key_padding_mask=mask, pos=pos_embed, query_pos=query_embed)
         return hs.transpose(1, 2), memory.permute(1, 2, 0).view(bs, c, h, w)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------------
+# the DETR tail: input_proj, class_embed, bbox_embed   (yolov7/modeling/meta_arch/detr.py:282-294, 406-472)
+# ------------------------------------------------------------------------------------------------------------------------------------
+def _pad16(n):
+    return (n + 15) // 16 * 16
+
+
+class _LinearStackFn(torch.autograd.Function):
+    """x [..., in] fp32 -> Linear (+ReLU) ... Linear -> [..., out] fp32, every row of x in one GEMM per layer (bf16 operands, fp32 bias and
+    accumulation).  The last layer's output channels are padded to a multiple of 16 for the GEMMs and sliced off.  Backward: ReLU-masked data
+    gradients with fused bias sums, weight gradients and column sums on the same kernels as the transformer layers."""
+
+    @staticmethod
+    def forward(ctx, kn, x, *params):
+        ws, bs = params[0::2], params[1::2]
+        lead, cin = x.shape[:-1], x.shape[-1]
+        if cin % 16 or any(w.shape[0] % 16 for w in ws[:-1]):
+            raise capi.Yb200Error(f"Linear stack: input {cin} and hidden widths {[w.shape[0] for w in ws[:-1]]} must be multiples of 16")
+        n = x.numel() // cin
+        h = x.detach().reshape(1, 1, n, cin).to(torch.bfloat16).contiguous()
+        hs, wds = [h], []
+        for i, (w, b) in enumerate(zip(ws, bs)):
+            last = i == len(ws) - 1
+            cout, cpad = w.shape[0], _pad16(w.shape[0])
+            wf = torch.empty(cpad, 1, w.shape[1], dtype=torch.bfloat16, device=x.device)
+            wd = torch.empty(w.shape[1], 1, cpad, dtype=torch.bfloat16, device=x.device)
+            capi.check(kn.L.yb200_pack_conv_weight(capi.ptr(w.detach().contiguous()), cout, w.shape[1], 1, cpad, w.shape[1], capi.ptr(wf), capi.ptr(wd),
+                                                   capi.stream_ptr()), "pack")
+            bias = torch.zeros(cpad, device=x.device)
+            bias[:cout] = b.detach()
+            out = torch.empty(1, 1, n, cpad, dtype=torch.bfloat16, device=x.device)
+            ha, oa = kn._a(h), kn._a(out)
+            if last:
+                capi.check(kn.L.yb200_conv2d_affine_fwd(ctypes.byref(ha), capi.ptr(wf), None, capi.ptr(bias), None, ctypes.byref(oa), 1, 1, capi.stream_ptr()),
+                           "linear")
+            else:
+                capi.check(kn.L.yb200_linear_relu_fwd(ctypes.byref(ha), capi.ptr(wf), capi.ptr(bias), ctypes.byref(oa), capi.stream_ptr()), "linear+relu")
+            wds.append(wd)
+            h = out
+            if not last:
+                hs.append(h)
+        ctx.kn, ctx.hs, ctx.wds, ctx.couts, ctx.lead, ctx.cin = kn, hs, wds, [w.shape[0] for w in ws], lead, cin
+        cout = ws[-1].shape[0]
+        return h[0, 0, :, :cout].float().reshape(*lead, cout)
+
+    @staticmethod
+    def backward(ctx, g):
+        kn, hs, wds, couts = ctx.kn, ctx.hs, ctx.wds, ctx.couts
+        n, dev = hs[0].shape[2], g.device
+        d = torch.zeros(1, 1, n, _pad16(couts[-1]), dtype=torch.bfloat16, device=dev)
+        d[0, 0, :, :couts[-1]] = g.reshape(n, couts[-1])
+        grads = [None] * (2 * len(couts))
+        gb = torch.empty(d.shape[-1], device=dev)
+        kn.colsum(d, gb)
+        grads[-1] = gb[:couts[-1]]
+        for i in range(len(couts) - 1, -1, -1):
+            gw = torch.empty(d.shape[-1], hs[i].shape[-1], device=dev)
+            kn.wgrad(hs[i], d, gw)
+            grads[2 * i] = gw[:couts[i]]
+            if i > 0:
+                d, grads[2 * i - 1] = kn.dgrad_relu(d, wds[i], hs[i])
+            else:
+                dx = kn.dgrad(d, wds[0], ctx.cin)
+        return (None, dx.float().reshape(*ctx.lead, ctx.cin)) + tuple(grads)
+
+
+def _linear_stack(kn, x, linears):
+    if not x.is_cuda:
+        raise capi.Yb200Error("DETR heads: inputs must be CUDA tensors (no CPU path)")
+    return _LinearStackFn.apply(kn, x, *[p for lin in linears for p in (lin.weight, lin.bias)])
+
+
+class MLP(nn.Module):
+    """detr.py:282-294: Linear + ReLU ... Linear over the last dimension, all rows in one GEMM per layer"""
+
+    def __init__(self, input_dim, hidden_dim, output_dim, num_layers):
+        super().__init__()
+        self.num_layers = num_layers
+        h = [hidden_dim] * (num_layers - 1)
+        self.layers = nn.ModuleList(nn.Linear(n, k) for n, k in zip([input_dim] + h, h + [output_dim]))
+        self.k = _Kernels()
+
+    def forward(self, x):
+        return _linear_stack(self.k, x, self.layers)
+
+
+class DETR(nn.Module):
+    """detr.py:406-472.  `backbone` is the caller's module, called as the reference calls it (features, pos = backbone(samples);
+    src, mask = features[-1].decompose()); `transformer` is this package's Transformer (return_intermediate_dec = deep supervision).
+    input_proj (1x1 convolution) and the heads run as GEMMs over every pixel / every (layer, image, query) row at once; pred_logits and
+    pred_boxes are fp32."""
+
+    def __init__(self, backbone, transformer, num_classes, num_queries, aux_loss=False):
+        super().__init__()
+        self.num_queries = num_queries
+        self.transformer = transformer
+        hidden_dim = transformer.d_model
+        self.class_embed = nn.Linear(hidden_dim, num_classes + 1)
+        self.bbox_embed = MLP(hidden_dim, hidden_dim, 4, 3)
+        self.query_embed = nn.Embedding(num_queries, hidden_dim)
+        self.input_proj = nn.Conv2d(backbone.num_channels, hidden_dim, kernel_size=1)
+        self.backbone = backbone
+        self.aux_loss = aux_loss
+        self.onnx_export = False
+        self.k = self.bbox_embed.k
+
+    def forward(self, samples):
+        if isinstance(samples, (list, torch.Tensor)):
+            raise capi.Yb200Error("DETR: pass a NestedTensor / ImageList with its padding mask (raw tensors and lists are not supported)")
+        features, pos = self.backbone(samples)
+        src, mask = features[-1].decompose()
+        assert mask is not None
+        conv = self.input_proj
+        proj_lin = types.SimpleNamespace(weight=conv.weight.view(conv.weight.shape[0], -1), bias=conv.bias)
+        proj = _linear_stack(self.k, src.permute(0, 2, 3, 1), [proj_lin]).permute(0, 3, 1, 2)
+        hs = self.transformer(proj, mask, self.query_embed.weight, pos[-1])[0]
+        outputs_class = _linear_stack(self.k, hs, [self.class_embed])
+        outputs_coord = torch.sigmoid(self.bbox_embed(hs))
+        out = {"pred_logits": outputs_class[-1], "pred_boxes": outputs_coord[-1]}
+        if self.aux_loss:
+            out["aux_outputs"] = [{"pred_logits": a, "pred_boxes": b} for a, b in zip(outputs_class[:-1], outputs_coord[:-1])]
+        return out

@@ -344,7 +344,9 @@ int yb200_conv2d_relu_fwd(const yb200_act* x, const void* w_fwd, const float* bi
  * `torch.bmm(pred_kernel, mask_features.view(B, C, HW))` (:143-146); cout <= 128                                                            */
 int yb200_conv1x1_nchw_f32(const yb200_act* x, const void* w_fwd, const float* bias, int cout, float* out_nchw, void* stream);
 /* The same for a whole batch with ONE WEIGHT MATRIX PER IMAGE (w_fwd: [x->n][cout][x->c] bf16 = the batch's predicted kernels): the batched
- * `torch.bmm` of :143-146 in one launch.  h * w must be a multiple of 128 pixels arranged so that a tile stays inside one image.            */
+ * `torch.bmm` of :143-146 in one launch.  Accepted when the 128-pixel tile choose_tile picks for (n, h, w) holds one image (tile width x
+ * height = 128: e.g. 80x80, 64x64, 72x96, any map at n = 1, and maps like 1x65 whose tiles overhang the image); otherwise (e.g. 40x40 or
+ * 60x80 at n = 2, two images per tile) YB200_ERR_UNSUPPORTED, the output untouched: call yb200_conv1x1_nchw_f32 per image.                */
 int yb200_conv1x1_nchw_f32_batched(const yb200_act* x, const void* w_fwd, int cout, float* out_nchw, void* stream);
 /* F.interpolate(x, scale_factor=2, mode="bilinear", align_corners=False) on fp32 planes [planes][h][w] -> [planes][2h][2w]: the mask logits
  * (:148-153)                                                                                                                                  */

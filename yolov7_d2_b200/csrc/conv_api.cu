@@ -447,7 +447,7 @@ extern "C" int yb200_linear_gelu_fwd(const yb200_act* x, const void* w_fwd, cons
 }
 
 // batched: one weight matrix PER IMAGE (w_fwd: [n][cout][cin] bf16, i.e. n * cout rows), torch.bmm(pred_kernel, mask_features) of a whole batch in
-// one launch.  Pixel tiles must not span images (h * w a multiple of the 128-pixel tile: choose_tile then keeps tiles inside one image).
+// one launch.  Pixel tiles must not span images: accepted when the tile choose_tile picks is 128 pixels of one image (width x height = 128).
 static int conv1x1_nchw_impl(const char* who, const yb200_act* x, const void* w_fwd, const float* bias, int cout, float* out_nchw, bool batched,
                              void* stream) {
   int rc;

@@ -432,6 +432,35 @@ int yb200_detr_set_loss_bwd(const float* logits, const float* boxes, const int32
                             const int32_t* offsets, int L, int B, int Q, int K1, float eos_coef, float num_boxes, const float* grad, float* dlogits,
                             float* dboxes, void* stream);
 
+/* ---- SparseInst matcher and criterion (yolov7/modeling/loss/sparseinst_loss.py) --------------------------------------------------------------
+ * pred_logits fp32 [B][N][K], pred_masks fp32 [B][N][H*W] (HW = H*W), pred_scores fp32 [B][N].  The targets of the batch are packed: labels int32
+ * [G], offsets int32 [B+1] (image b owns targets [offsets[b], offsets[b+1]), offsets[B] = G), the resized masks tmasks fp32 [G][HW] and their
+ * Σt² tsq [G] (yb200_sparseinst_target_masks).  labels / tmasks / tsq must not be NULL even when G = 0.  N <= 4096, B*N < 65536.
+ *   yb200_sparseinst_target_masks: masks = the uint8 masks of the batch in one buffer; table int64 [G][3] = (byte offset, h, w) of each.  out
+ *     [G][H][W] = the mask zero-padded to in_h x in_w (nested_masks_from_list, :320-322) and resized by F.interpolate(bilinear,
+ *     align_corners=False) (:326-331) with ATen's index and weight formula; tsq[g] = Σ out[g]².  Every mask needs h <= in_h, w <= in_w.
+ *   yb200_sparseinst_match_cost: SparseInstMatcher's C = dice^alpha * sigmoid(logit[label])^beta (:336-340), dice = 2 Σσ(m)t / (Σσ(m)² + Σt² +
+ *     1e-4), only the per-image blocks: block b is [N][G_b] row-major at cost + N*offsets[b].  cost has N*G + 1 floats: the last one is an int32
+ *     status word, bit 0 = a label outside [0, K), bit 1 = an image with more than N targets (its block is not written).
+ *   yb200_sparseinst_set_loss: match int32 [B][N] = the matched target's index within its image, or -1; num_pairs = matched rows.  out fp32 [4]
+ *     = (loss_ce, loss_objectness, loss_dice, loss_mask) weighted by (w_ce, w_obj, w_dice, w_mask), as loss_labels and
+ *     loss_masks_with_iou_objectness (:89-184) compute them; the three mask terms are 0 when num_pairs = 0.  save fp32 [B][N][8]: per-row sums
+ *     the backward reads.
+ *   yb200_sparseinst_set_loss_bwd: grad fp32 [4] = upstream gradients of out (device memory); writes dlogits [B][N][K], dmasks [B][N][HW] (zero
+ *     on unmatched rows) and dscores [B][N] (zero on unmatched rows).  The IoU target carries no gradient.
+ * Fixed summation order (bit-reproducible), no host synchronisation.                                                                            */
+int yb200_sparseinst_target_masks(const uint8_t* masks, const int64_t* table, int G, int in_h, int in_w, int H, int W, float* out, float* tsq,
+                                  void* stream);
+int yb200_sparseinst_match_cost(const float* logits, const float* masks, const int32_t* labels, const int32_t* offsets, const float* tmasks,
+                                const float* tsq, int B, int N, int K, int HW, int G, float alpha, float beta, float* cost, void* stream);
+int yb200_sparseinst_set_loss(const float* logits, const float* masks, const float* scores, const int32_t* match, const int32_t* labels,
+                              const int32_t* offsets, const float* tmasks, const float* tsq, int B, int N, int K, int HW, int num_pairs, float w_ce,
+                              float w_obj, float w_dice, float w_mask, float num_instances, float* save, float* out, void* stream);
+int yb200_sparseinst_set_loss_bwd(const float* logits, const float* masks, const float* scores, const int32_t* match, const int32_t* labels,
+                                  const int32_t* offsets, const float* tmasks, const float* tsq, const float* save, int B, int N, int K, int HW,
+                                  int num_pairs, float w_ce, float w_obj, float w_dice, float w_mask, float num_instances, const float* grad,
+                                  float* dlogits, float* dmasks, float* dscores, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -146,3 +146,38 @@ def detr_set_loss_bwd(logits, boxes, match, labels, target_boxes, offsets, eos_c
     check(lib().yb200_detr_set_loss_bwd(_f32(logits), _f32(boxes), _i32(match), _i32(labels), _f32(target_boxes), _i32(offsets), L, B, Q, K1,
                                         c_float(eos_coef), c_float(num_boxes), _f32(grad), _f32(dlogits), _f32(dboxes), stream_ptr()),
           "detr_set_loss_bwd")
+
+
+def sparseinst_target_masks(masks, table, num_targets, input_shape, size, out, tsq):
+    """yb200_sparseinst_target_masks on the current stream: packed uint8 masks + int64 [G, 3] table -> out [G, H, W], tsq [G]"""
+    assert masks.dtype == torch.uint8 and table.dtype == torch.int64 and table.is_contiguous()
+    check(lib().yb200_sparseinst_target_masks(ptr(masks), ptr(table), num_targets, int(input_shape[0]), int(input_shape[1]), int(size[0]), int(size[1]),
+                                              _f32(out), _f32(tsq), stream_ptr()), "sparseinst_target_masks")
+
+
+def sparseinst_match_cost(logits, masks, labels, offsets, tmasks, tsq, num_targets, alpha, beta, cost):
+    """yb200_sparseinst_match_cost on the current stream: logits [B, N, K], masks [B, N, H, W] -> cost (N*G floats + the status word)"""
+    B, N, K = logits.shape
+    check(lib().yb200_sparseinst_match_cost(_f32(logits), _f32(masks), _i32(labels), _i32(offsets), _f32(tmasks), _f32(tsq), B, N, K,
+                                            masks.shape[-2] * masks.shape[-1], num_targets, c_float(alpha), c_float(beta), _f32(cost), stream_ptr()),
+          "sparseinst_match_cost")
+
+
+def sparseinst_set_loss(logits, masks, scores, match, labels, offsets, tmasks, tsq, num_pairs, weights, num_instances, save, out):
+    """yb200_sparseinst_set_loss on the current stream: out [4] = weighted (loss_ce, loss_objectness, loss_dice, loss_mask); save [B, N, 8]"""
+    B, N, K = logits.shape
+    w_ce, w_obj, w_dice, w_mask = (c_float(w) for w in weights)
+    check(lib().yb200_sparseinst_set_loss(_f32(logits), _f32(masks), _f32(scores), _i32(match), _i32(labels), _i32(offsets), _f32(tmasks), _f32(tsq), B, N,
+                                          K, masks.shape[-2] * masks.shape[-1], num_pairs, w_ce, w_obj, w_dice, w_mask, c_float(num_instances),
+                                          _f32(save), _f32(out), stream_ptr()), "sparseinst_set_loss")
+
+
+def sparseinst_set_loss_bwd(logits, masks, scores, match, labels, offsets, tmasks, tsq, save, num_pairs, weights, num_instances, grad, dlogits, dmasks,
+                            dscores):
+    """yb200_sparseinst_set_loss_bwd on the current stream: grad [4] (device) -> dlogits, dmasks, dscores shaped like logits, masks, scores"""
+    B, N, K = logits.shape
+    w_ce, w_obj, w_dice, w_mask = (c_float(w) for w in weights)
+    check(lib().yb200_sparseinst_set_loss_bwd(_f32(logits), _f32(masks), _f32(scores), _i32(match), _i32(labels), _i32(offsets), _f32(tmasks), _f32(tsq),
+                                              _f32(save), B, N, K, masks.shape[-2] * masks.shape[-1], num_pairs, w_ce, w_obj, w_dice, w_mask,
+                                              c_float(num_instances), _f32(grad), _f32(dlogits), _f32(dmasks), _f32(dscores), stream_ptr()),
+          "sparseinst_set_loss_bwd")

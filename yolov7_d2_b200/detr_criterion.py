@@ -18,6 +18,16 @@ from . import capi
 STATUS_BAD_LABEL, STATUS_BAD_BOX = 1, 2  # bits of the status word written by yb200_detr_match_cost
 
 
+def num_per_rank(total, device):
+    """the target count normalising the losses, averaged over the ranks and clamped to >= 1 (detr.py:620-624, sparseinst_loss.py:204-212);
+    without a process group it is known on the host and costs no synchronisation"""
+    if dist.is_available() and dist.is_initialized():
+        nb = torch.as_tensor([total], dtype=torch.float, device=device)
+        dist.all_reduce(nb)
+        return torch.clamp(nb / dist.get_world_size(), min=1).item()
+    return float(max(total, 1))
+
+
 class _Targets:
     """the batch's targets packed for the kernels: labels int32 [G], boxes fp32 [G, 4], offsets int32 [B + 1] (device), sizes (host)"""
 
@@ -135,14 +145,6 @@ class SetCriterion(nn.Module):
         empty_weight[-1] = self.eos_coef
         self.register_buffer("empty_weight", empty_weight)
 
-    def _num_boxes(self, total, device):
-        """detr.py:620-624; without a process group it is known on the host and costs no synchronisation"""
-        if dist.is_available() and dist.is_initialized():
-            nb = torch.as_tensor([total], dtype=torch.float, device=device)
-            dist.all_reduce(nb)
-            return torch.clamp(nb / dist.get_world_size(), min=1).item()
-        return float(max(total, 1))
-
     def forward(self, outputs, targets):
         for loss in self.losses:
             if loss == "masks":
@@ -165,7 +167,7 @@ class SetCriterion(nn.Module):
         tg = _Targets(targets, device)
         _, match_host = self.matcher.match_layers(logits, boxes, tg)
         match = match_host.to(device, non_blocking=True)
-        num_boxes = self._num_boxes(tg.total, device)
+        num_boxes = num_per_rank(tg.total, device)
         out = _SetLossFn.apply((logits, boxes, match, tg, float(self.eos_coef), num_boxes), *logits_in, *boxes_in)
         stats = out.detach()
         L = len(layers)

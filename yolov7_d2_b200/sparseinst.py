@@ -12,7 +12,8 @@ Kernel sequence (NHWC bf16 inside):
   heads: three small GEMMs with fp32 output (`yb200_conv1x1_bias_f32`)  |  mask projection 1x1
   pred_masks = per-image 1x1 convolution of the mask features with pred_kernel[b] as weights, fp32 NCHW written by the GEMM epilogue
 The final bilinear x2 up-sampling (decoder_sparseinst.py:148-153) is `yb200_upsample_bilinear2x_f32` (other scale factors: F.interpolate).
-Round-1 scope: forward (inference; the loss / Hungarian matching of sparseinst_loss.py and the backward are not built): runs under no_grad.
+Scope: forward (inference; the decoder backward is not built): runs under no_grad.  The matcher and the losses of sparseinst_loss.py, with
+their gradients w.r.t. this module's outputs, are `sparseinst_criterion.py`.
 Instance / kernel counts are padded to multiples of 16 internally (100 -> 112: padded IAM channels get bias -30, i.e. probability 0).
 """
 import ctypes

@@ -29,9 +29,12 @@ def test_encoder_layer_matches_reference(cuda):
     layer = TransformerEncoderLayer(d, nhead, dim_feedforward=ffn, dropout=0.0)
     layer.load_state_dict({k: v.to(cuda) for k, v in dto.layer_state_dict("encoder", d, ffn, seed=2).items()}, strict=True)
     layer.eval()
-    out = layer(torch.tensor(gold["enc_src"]).to(cuda), src_key_padding_mask=torch.tensor(gold["enc_mask"]).to(cuda), pos=torch.tensor(gold["enc_pos"]).to(cuda))
+    args = torch.tensor(gold["enc_src"]).to(cuda), torch.tensor(gold["enc_mask"]).to(cuda), torch.tensor(gold["enc_pos"]).to(cuda)
+    out = layer(args[0], src_key_padding_mask=args[1], pos=args[2])
     assert out.shape == (L, b, d) and out.dtype == torch.float32
     _check(out, gold["enc_out"], "encoder layer output")
+    with torch.no_grad():
+        _check(layer(args[0], src_key_padding_mask=args[1], pos=args[2]), gold["enc_out"], "encoder layer output (no grad)")
     # without mask / positional embedding: against the oracle (pinned to the reference by tests/test_detr_oracle_golden.py)
     sd = {"l." + k: v for k, v in dto.layer_state_dict("encoder", d, ffn, seed=2).items()}
     src = torch.tensor(gold["enc_src"])
@@ -49,11 +52,14 @@ def test_decoder_layer_matches_reference(cuda):
     t = lambda k: torch.tensor(gold[k]).to(cuda)
     out = layer(t("dec_tgt"), t("dec_mem"), memory_key_padding_mask=t("enc_mask"), pos=t("enc_pos"), query_pos=t("dec_qpos"))
     _check(out, gold["dec_out"], "decoder layer output")
+    with torch.no_grad():
+        out = layer(t("dec_tgt"), t("dec_mem"), memory_key_padding_mask=t("enc_mask"), pos=t("enc_pos"), query_pos=t("dec_qpos"))
+    _check(out, gold["dec_out"], "decoder layer output (no grad)")
 
 
 def test_layers_refuse_what_is_not_built(cuda):
     from yolov7_d2_b200 import capi
-    from yolov7_d2_b200.detr import TransformerEncoderLayer
+    from yolov7_d2_b200.detr import TransformerDecoderLayer, TransformerEncoderLayer
 
     with pytest.raises(capi.Yb200Error):
         TransformerEncoderLayer(96, 2)  # head dimension 48
@@ -62,6 +68,20 @@ def test_layers_refuse_what_is_not_built(cuda):
         layer(torch.randn(10, 1, 64))  # CPU tensor
     with pytest.raises(capi.Yb200Error):
         layer(torch.randn(10, 1, 64, device=cuda), src_mask=torch.zeros(10, 10, device=cuda))
+    # every tensor argument is checked before any kernel sees its pointer, with and without autograd
+    src = torch.randn(10, 1, 64, device=cuda)
+    with pytest.raises(capi.Yb200Error, match="CUDA tensors"):
+        layer(src, pos=torch.randn(10, 1, 64))
+    with pytest.raises(capi.Yb200Error, match="CUDA tensors"):
+        layer(src, src_key_padding_mask=torch.zeros(1, 10, dtype=torch.bool))
+    dec = TransformerDecoderLayer(64, 2, dim_feedforward=128)
+    tgt, mem = torch.randn(6, 1, 64, device=cuda), torch.randn(10, 1, 64, device=cuda)
+    with pytest.raises(capi.Yb200Error, match="CUDA tensors"):
+        dec(tgt, torch.randn(10, 1, 64))
+    with pytest.raises(capi.Yb200Error, match="CUDA tensors"):
+        dec(tgt, mem, query_pos=torch.randn(6, 1, 64))
+    with torch.no_grad(), pytest.raises(capi.Yb200Error, match="CUDA tensors"):
+        dec(tgt, mem, memory_key_padding_mask=torch.zeros(1, 10, dtype=torch.bool))
 
 
 def test_relu_epilogues(cuda):

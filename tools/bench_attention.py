@@ -54,6 +54,10 @@ tgt, qpos = torch.randn(100, b, e, device=dev), torch.randn(100, b, e, device=de
 mask = torch.zeros(b, l, dtype=torch.bool, device=dev)
 res["encoder layer forward (bs16, 1050 tokens, FFN 2048)"] = {"us": timeit(lambda: enc(src, src_key_padding_mask=mask, pos=pos), 10) * 1e3}
 res["decoder layer forward (100 queries)"] = {"us": timeit(lambda: dec(tgt, src, memory_key_padding_mask=mask, pos=pos, query_pos=qpos), 10) * 1e3}
+# inference: the same layers without autograd (no log-sum-exp or LayerNorm statistics kept)
+with torch.no_grad():
+    res["encoder layer forward, no grad"] = {"us": timeit(lambda: enc(src, src_key_padding_mask=mask, pos=pos), 10) * 1e3}
+    res["decoder layer forward, no grad (100 queries)"] = {"us": timeit(lambda: dec(tgt, src, memory_key_padding_mask=mask, pos=pos, query_pos=qpos), 10) * 1e3}
 # training: layer forward + backward through autograd (the kernels' own backward wiring, detr._EncoderLayerFn / _DecoderLayerFn), and the 6 + 6 stack
 from yolov7_d2_b200.detr import Transformer
 enc.train(); dec.train()

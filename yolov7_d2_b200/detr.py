@@ -8,9 +8,11 @@ constructor arguments, parameter names / shapes (`self_attn.in_proj_weight` [3E,
     x (+pos) -> in_proj GEMMs (bias epilogue, q|k|v packed in one [B, L, 3E] buffer) -> yb200_attention_fwd (wgmma, streaming softmax)
       -> out_proj GEMM (+bias +residual epilogue) -> LayerNorm -> linear1 GEMM (+bias +ReLU epilogue) -> linear2 GEMM (+bias +residual) -> LayerNorm
 
-Internally tokens are batch-first bf16 `[B, 1, L, E]` views (yb200_act).  Forward and backward: with gradients enabled the layers run as one autograd node each
-(`_EncoderLayerFn` / `_DecoderLayerFn`: attention backward, data / weight gradients and LayerNorm backward on the same kernels), validated on
-hardware against the reference layer's autograd (tests/test_detr_gpu.py); YB200_DETR_TRAINING=0 forces the inference path.
+Internally tokens are batch-first bf16 `[B, 1, L, E]` views (yb200_act).  Each layer is built from two blocks, each with one forward and one
+backward: the attention block (`_attention_fwd` / `_attention_bwd`, self- or cross-attention) and the FFN block (`_ffn_fwd` / `_ffn_bwd`).
+With gradients enabled the layers run as one autograd node each (`_EncoderLayerFn` / `_DecoderLayerFn`: attention backward, data / weight
+gradients and LayerNorm backward on the same kernels), validated on hardware against the reference layer's autograd (tests/test_detr_gpu.py);
+without autograd they run the same block forwards without keeping the log-sum-exp or the LayerNorm statistics.
 Dropout (p = 0.1 in the reference: on the attention probabilities inside nn.MultiheadAttention and nn.Dropout on the residual branches / in the FFN) is
 active in training mode: the masks are a counter-based hash of (seed, element index) evaluated inside the kernels (yb200_attention_*_dropout,
 yb200_dropout), regenerated in the backward from the same seeds; seeds come from torch's CPU generator.  Same distribution as torch's Philox masks, not
@@ -18,7 +20,7 @@ the same bits: parity = the same computation given the same mask (tests/test_det
 reference's DETR) and `normalize_before=True` are not supported.  There is no CPU implementation.
 """
 import ctypes
-import os
+import operator
 import types
 
 import torch
@@ -27,9 +29,8 @@ import torch.nn as nn
 from . import capi
 
 LN_EPS = 1e-5
-# The layers' backward wiring (autograd.Function over the attention-backward / dgrad / wgrad / LayerNorm-backward kernels) is the default
-# whenever autograd is recording; YB200_DETR_TRAINING=0 switches it off (inference-only modules)
-TRAINING_PATH = os.environ.get("YB200_DETR_TRAINING", "1") == "1"
+# (p, seeds) of a forward without autograd: it runs dropout-free, and draws no seeds from torch's generator
+_NO_DROPOUT = (0.0, (0,) * 6)
 
 
 def _bl(t):
@@ -40,6 +41,10 @@ def _bl(t):
 def _lb(t):
     """[B, 1, L, E] bf16 -> [L, B, E] fp32"""
     return t.squeeze(1).permute(1, 0, 2).float().contiguous()
+
+
+def _f32(*shape, device):
+    return torch.empty(*shape, device=device)
 
 
 class _Kernels:
@@ -58,6 +63,15 @@ class _Kernels:
         capi.check(self.L.yb200_pack_conv_weight(capi.ptr(w.detach().contiguous()), out_f, in_f, 1, out_f, in_f, capi.ptr(wf), None, capi.stream_ptr()), "pack")
         return wf
 
+    def pack2(self, w, rows=None):
+        """[out, in] fp32 -> bf16 forward [rows, 1, in] and data-gradient [in, 1, rows] GEMM operands; rows > out pads with zero rows"""
+        out_f, in_f = w.shape
+        rows = out_f if rows is None else rows
+        wf = torch.empty(rows, 1, in_f, dtype=torch.bfloat16, device=w.device)
+        wd = torch.empty(in_f, 1, rows, dtype=torch.bfloat16, device=w.device)
+        capi.check(self.L.yb200_pack_conv_weight(capi.ptr(w.detach().contiguous()), out_f, in_f, 1, rows, in_f, capi.ptr(wf), capi.ptr(wd), capi.stream_ptr()), "pack")
+        return wf, wd
+
     def add(self, a, b):
         out = torch.empty_like(a)
         aa, ba, oa = self._a(a), self._a(b), self._a(out)
@@ -65,14 +79,15 @@ class _Kernels:
         return out
 
     def linear(self, x, w, bias, out=None, out_off=0, residual=None, relu=False):
-        """out[..., out_off:out_off+N] = x W^T + bias (+ residual) (ReLU); x may be a (tensor, off, c) slice"""
+        """out[..., out_off:out_off+N] = x W^T + bias (+ residual) (ReLU); x may be a (tensor, off, c) slice; w is an [N, in] fp32 weight or the
+        forward operand from pack2"""
         xt, xo, xc = x if isinstance(x, tuple) else (x, 0, None)
         n_out = w.shape[0]
         b, _, l, _ = xt.shape
         if out is None:
             out = torch.empty(b, 1, l, n_out, dtype=torch.bfloat16, device=xt.device)
         xa, oa = self._a(xt, xo, xc), self._a(out, out_off, n_out)
-        wf = self.pack(w)
+        wf = w if w.dim() == 3 else self.pack(w)
         bias = bias.detach().contiguous()
         if relu:
             capi.check(self.L.yb200_linear_relu_fwd(ctypes.byref(xa), capi.ptr(wf), capi.ptr(bias), ctypes.byref(oa), capi.stream_ptr()), "linear+relu")
@@ -82,32 +97,22 @@ class _Kernels:
                                                       ctypes.byref(oa), 1, 1, capi.stream_ptr()), "linear")
         return out
 
-    def layernorm(self, x, weight, bias):
-        y = torch.empty_like(x)
-        xa, ya = self._a(x), self._a(y)
-        capi.check(self.L.yb200_layernorm_fwd(ctypes.byref(xa), capi.ptr(weight.detach().contiguous()), capi.ptr(bias.detach().contiguous()), ctypes.c_float(LN_EPS),
-                                              ctypes.byref(ya), None, capi.stream_ptr()), "layernorm")
-        return y
-
-    # ---- helpers of the training path ------------------------------------------------------------------------------------------
-    def pack2(self, w):
-        out_f, in_f = w.shape
-        wf = torch.empty(out_f, 1, in_f, dtype=torch.bfloat16, device=w.device)
-        wd = torch.empty(in_f, 1, out_f, dtype=torch.bfloat16, device=w.device)
-        capi.check(self.L.yb200_pack_conv_weight(capi.ptr(w.detach().contiguous()), out_f, in_f, 1, out_f, in_f, capi.ptr(wf), capi.ptr(wd), capi.stream_ptr()), "pack")
-        return wf, wd
-
-    def _ws(self, nbytes, dev):
-        return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=dev)
-
-    def layernorm_train(self, x, weight, bias):
+    def layernorm(self, x, weight, bias, save=False):
+        """save: also return the per-row (mean, rstd) that layernorm_bwd needs (else None)"""
         b, _, l, _ = x.shape
         y = torch.empty_like(x)
-        stats = torch.empty(b * l, 2, device=x.device)
+        stats = torch.empty(b * l, 2, device=x.device) if save else None
         xa, ya = self._a(x), self._a(y)
         capi.check(self.L.yb200_layernorm_fwd(ctypes.byref(xa), capi.ptr(weight.detach().contiguous()), capi.ptr(bias.detach().contiguous()), ctypes.c_float(LN_EPS),
                                               ctypes.byref(ya), capi.ptr(stats), capi.stream_ptr()), "layernorm")
         return y, stats
+
+    def layernorm_train(self, x, weight, bias):
+        """the forward of the autograd path: keeps the statistics"""
+        return self.layernorm(x, weight, bias, save=True)
+
+    def _ws(self, nbytes, dev):
+        return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=dev)
 
     def layernorm_bwd(self, dy, x, stats, weight):
         dx = torch.empty_like(x)
@@ -158,16 +163,22 @@ class _Kernels:
         ws = self._ws(self.L.yb200_colsum_workspace(ctypes.byref(da)), dt.device)
         capi.check(self.L.yb200_colsum(ctypes.byref(da), ctypes.c_float(1.0), capi.ptr(out), 0, capi.ptr(ws), capi.stream_ptr()), "colsum")
 
-    def attention_train(self, q, k, v, mask, heads, p_drop=0.0, seed=0):
-        """p_drop > 0: dropout on the attention probabilities (nn.MultiheadAttention(dropout=p), detr_backbone.py:140), mask = f(seed, b, h, q, k)"""
+    def attention(self, q, k, v, mask, heads, p_drop=0.0, seed=0, save=False):
+        """q, k, v: (tensor, channel offset, E) slices of [B,1,L,*] buffers; mask: uint8 [B, Lk] or None.  p_drop > 0: dropout on the attention
+        probabilities (nn.MultiheadAttention(dropout=p), detr_backbone.py:140), mask = f(seed, b, h, q, k).  save: also return the log-sum-exp
+        that attention_bwd needs (else None)"""
         qt, _, e = q
         b, _, lq, _ = qt.shape
         out = torch.empty(b, 1, lq, e, dtype=torch.bfloat16, device=qt.device)
-        lse = torch.empty(b, heads, lq, device=qt.device)
+        lse = torch.empty(b, heads, lq, device=qt.device) if save else None
         qa, ka, va, oa = self._a(*q), self._a(*k), self._a(*v), self._a(out)
         capi.check(self.L.yb200_attention_fwd_dropout(ctypes.byref(qa), ctypes.byref(ka), ctypes.byref(va), capi.ptr(mask), ctypes.c_float((e // heads) ** -0.5),
                                                       ctypes.byref(oa), capi.ptr(lse), ctypes.c_float(p_drop), ctypes.c_uint32(seed), capi.stream_ptr()), "attention")
         return out, lse
+
+    def attention_train(self, q, k, v, mask, heads, p_drop=0.0, seed=0):
+        """the forward of the autograd path: keeps the log-sum-exp"""
+        return self.attention(q, k, v, mask, heads, p_drop, seed, save=True)
 
     def attention_bwd(self, q, k, v, out, dout, mask, heads, lse, dq, dk, dv, p_drop=0.0, seed=0):
         e = q[2]
@@ -188,25 +199,19 @@ class _Kernels:
                                         ctypes.c_float(scale), capi.stream_ptr()), "dropout")
         return out
 
-    def attention(self, q, k, v, mask, heads):
-        """q, k, v: (tensor, channel offset, E) slices of [B,1,L,*] buffers; mask: uint8 [B, Lk] or None"""
-        qt, qo, e = q
-        b, _, lq, _ = qt.shape
-        out = torch.empty(b, 1, lq, e, dtype=torch.bfloat16, device=qt.device)
-        qa, ka, va, oa = self._a(*q), self._a(*k), self._a(*v), self._a(out)
-        capi.check(self.L.yb200_attention_fwd(ctypes.byref(qa), ctypes.byref(ka), ctypes.byref(va), capi.ptr(mask), ctypes.c_float((e // heads) ** -0.5),
-                                              ctypes.byref(oa), None, capi.stream_ptr()), "attention")
-        return out
+
+def _check_devices(*tensors):
+    """the kernels take raw device pointers: every tensor argument of a layer is a CUDA tensor, all on one device"""
+    devices = {t.device for t in tensors if t is not None}
+    if any(d.type != "cuda" for d in devices):
+        raise capi.Yb200Error("DETR layers: inputs must be CUDA tensors (no CPU path)")
+    if len(devices) > 1:
+        raise capi.Yb200Error(f"DETR layers: inputs on more than one device ({', '.join(sorted(map(str, devices)))})")
 
 
-def _check_inputs(*tensors):
-    for t in tensors:
-        if t is None:
-            continue
-        if not t.is_cuda:
-            raise capi.Yb200Error("DETR layers: inputs must be CUDA tensors (no CPU path)")
-        if t.requires_grad and torch.is_grad_enabled():
-            raise capi.Yb200Error("DETR layers: the attention backward kernel is not built yet -- run under torch.no_grad()")
+def _records(*tensors):
+    """autograd is recording and one of the tensors requires grad: the layer runs as one autograd node"""
+    return torch.is_grad_enabled() and any(t.requires_grad for t in tensors)
 
 
 def _mask_u8(mask):
@@ -267,227 +272,191 @@ class _LayerBase(nn.Module):
             return 0.0, (0,) * n
         return p, tuple(int(v) for v in torch.randint(0, 2 ** 31 - 1, (n,)))
 
-    def _self_attention(self, x, qk, att, mask):
-        """x: value source, qk: query/key source ([B,1,L,E] bf16); returns x + out_proj(attention)"""
-        e, kn = self.d_model, self.k
-        b, _, l, _ = x.shape
-        qkv = torch.empty(b, 1, l, 3 * e, dtype=torch.bfloat16, device=x.device)
-        w, bias = att.in_proj_weight, att.in_proj_bias
-        kn.linear(qk, w[:2 * e], bias[:2 * e], out=qkv, out_off=0)
-        kn.linear(x, w[2 * e:], bias[2 * e:], out=qkv, out_off=2 * e)
-        a = kn.attention((qkv, 0, e), (qkv, e, e), (qkv, 2 * e, e), mask, self.nhead)
-        return kn.linear(a, att.out_proj.weight, att.out_proj.bias, residual=x)
 
-    def _ffn(self, x, norm):
-        kn = self.k
-        h = kn.linear(x, self.linear1.weight, self.linear1.bias, relu=True)
-        y = kn.linear(h, self.linear2.weight, self.linear2.bias, residual=x)
-        return kn.layernorm(y, norm.weight, norm.bias)
+# ------------------------------------------------------------------------------------------------------------------------------------
+# the blocks of forward_post (detr_backbone.py:157-170, 221-242).  A forward returns its output and, with save, what its backward needs
+# (the block's parameters, dropout state and bf16 intermediates); a backward returns the input gradients and the parameter gradients.
+# p = (in / linear1 weight, bias, out_proj / linear2 weight, bias, LayerNorm weight, bias); seeds = the block's two dropout seeds.
+# ------------------------------------------------------------------------------------------------------------------------------------
+def _linear_residual(kn, x, w, b, res, pd, seed):
+    """res + dropout(x W^T + b): the residual joins in the GEMM epilogue, or in the dropout kernel when p > 0"""
+    if pd > 0:
+        return kn.dropout(kn.linear(x, w, b), pd, seed, residual=res)
+    return kn.linear(x, w, b, residual=res)
+
+
+def _attention_fwd(kn, heads, x, q_src, kv_src, mask, p, pd, seeds, save):
+    """in-projection GEMMs -> attention core (dropout seeds[0]) -> out_proj (dropout seeds[1]) + residual x -> LayerNorm.
+    Self-attention (kv_src None): q|k from q_src in one [.., 2E] GEMM and v from x, into one [.., 3E] buffer.
+    Cross-attention (kv_src = (key source, value source)): q from q_src on its own, k and v into one [.., 2E] buffer."""
+    w, b, w_o, b_o, g, be = p
+    bs, _, lq, e = x.shape
+    if kv_src is None:
+        qkv = torch.empty(bs, 1, lq, 3 * e, dtype=torch.bfloat16, device=x.device)
+        kn.linear(q_src, w[:2 * e], b[:2 * e], out=qkv, out_off=0)
+        kn.linear(x, w[2 * e:], b[2 * e:], out=qkv, out_off=2 * e)
+        qkv_s = ((qkv, 0, e), (qkv, e, e), (qkv, 2 * e, e))
+    else:
+        k_src, v_src = kv_src
+        qc = kn.linear(q_src, w[:e], b[:e])
+        kv = torch.empty(bs, 1, k_src.shape[2], 2 * e, dtype=torch.bfloat16, device=x.device)
+        kn.linear(k_src, w[e:2 * e], b[e:2 * e], out=kv, out_off=0)
+        kn.linear(v_src, w[2 * e:], b[2 * e:], out=kv, out_off=e)
+        qkv_s = ((qc, 0, e), (kv, 0, e), (kv, e, e))
+    att, lse = (kn.attention_train if save else kn.attention)(*qkv_s, mask, heads, pd, seeds[0])
+    y = _linear_residual(kn, att, w_o, b_o, x, pd, seeds[1])
+    out, st = (kn.layernorm_train if save else kn.layernorm)(y, g, be)
+    return out, ((p, pd, seeds, mask, x, q_src, kv_src, qkv_s, att, lse, y, st) if save else None)
+
+
+def _attention_bwd(kn, heads, g, saved):
+    """-> (gradient of x, gradient of q_src, for cross-attention (gradient of the value source, gradient of the key source) else None,
+    parameter gradients).  x feeds the residual and the queries (q_src = x + query / positional embedding), and self-attention's keys and
+    values; the value source of cross-attention also feeds its keys (key source = value source + pos), so its gradient includes the key source's."""
+    (w, _, w_o, _, g_ln, _), pd, seeds, mask, x, q_src, kv_src, (q, k, v), att, lse, y, st = saved
+    e, dev = x.shape[-1], x.device
+    g_y, gg, gbe = kn.layernorm_bwd(g, y, st, g_ln)
+    g_o = kn.dropout(g_y, pd, seeds[1]) if pd > 0 else g_y
+    g_att = kn.dgrad(g_o, kn.pack2(w_o)[1], e)
+    gwo, gbo = _f32(e, e, device=dev), _f32(e, device=dev)
+    kn.wgrad(att, g_o, gwo)
+    kn.colsum(g_o, gbo)
+    gw, gb = _f32(3 * e, e, device=dev), _f32(3 * e, device=dev)
+    if kv_src is None:
+        dqkv = torch.empty_like(q[0])
+        kn.attention_bwd(q, k, v, att, g_att, mask, heads, lse, (dqkv, 0, e), (dqkv, e, e), (dqkv, 2 * e, e), pd, seeds[0])
+        g_q = kn.dgrad((dqkv, 0, 2 * e), kn.pack2(w[:2 * e])[1], e)
+        g_x = kn.add(kn.dgrad((dqkv, 2 * e, e), kn.pack2(w[2 * e:])[1], e, addend=g_y), g_q)
+        kn.wgrad(q_src, (dqkv, 0, 2 * e), gw[:2 * e])
+        kn.wgrad(x, (dqkv, 2 * e, e), gw[2 * e:])
+        kn.colsum(dqkv, gb)
+        g_kv = None
+    else:
+        k_src, v_src = kv_src
+        dqc, dkv = torch.empty_like(q[0]), torch.empty_like(k[0])
+        kn.attention_bwd(q, k, v, att, g_att, mask, heads, lse, (dqc, 0, e), (dkv, 0, e), (dkv, e, e), pd, seeds[0])
+        g_q = kn.dgrad(dqc, kn.pack2(w[:e])[1], e)
+        g_k = kn.dgrad((dkv, 0, e), kn.pack2(w[e:2 * e])[1], e)
+        g_kv = (kn.dgrad((dkv, e, e), kn.pack2(w[2 * e:])[1], e, addend=g_k), g_k)
+        kn.wgrad(q_src, dqc, gw[:e])
+        kn.wgrad(k_src, (dkv, 0, e), gw[e:2 * e])
+        kn.wgrad(v_src, (dkv, e, e), gw[2 * e:])
+        kn.colsum(dqc, gb[:e])
+        kn.colsum(dkv, gb[e:])
+        g_x = kn.add(g_y, g_q)
+    return g_x, g_q, g_kv, (gw, gb, gwo, gbo, gg, gbe)
+
+
+def _ffn_fwd(kn, x, p, pd, seeds, save):
+    """linear1 + ReLU (dropout seeds[0]) -> linear2 (dropout seeds[1]) + residual x -> LayerNorm"""
+    w1, b1, w2, b2, g, be = p
+    h = kn.linear(x, w1, b1, relu=True)
+    if pd > 0:
+        h = kn.dropout(h, pd, seeds[0])  # the dropped activation is what linear2 sees and what the backward needs (h > 0 and kept)
+    y = _linear_residual(kn, h, w2, b2, x, pd, seeds[1])
+    out, st = (kn.layernorm_train if save else kn.layernorm)(y, g, be)
+    return out, ((p, pd, seeds, x, h, y, st) if save else None)
+
+
+def _ffn_bwd(kn, g, saved):
+    """-> (gradient of x, parameter gradients)"""
+    (w1, _, w2, _, g_ln, _), pd, seeds, x, h, y, st = saved
+    e, ff, dev = x.shape[-1], w1.shape[0], x.device
+    g_y, gg, gbe = kn.layernorm_bwd(g, y, st, g_ln)
+    # linear2 and the ReLU in front of it; with dropout: g_t = the output dropout's mask on the branch gradient, and the saved h is the dropped
+    # activation (positive <=> positive and kept), so the ReLU mask also applies the FFN dropout mask -- its 1 / (1 - p) follows
+    g_t = kn.dropout(g_y, pd, seeds[1]) if pd > 0 else g_y
+    du, gb1 = kn.dgrad_relu(g_t, kn.pack2(w2)[1], h)
+    if pd > 0:
+        du = kn.dropout(du, pd, seeds[0])
+        gb1 = gb1 / (1.0 - pd)
+    gw2, gb2 = _f32(e, ff, device=dev), _f32(e, device=dev)
+    kn.wgrad(h, g_t, gw2)
+    kn.colsum(g_t, gb2)
+    # linear1; the residual branch of x joins through the addend
+    g_x = kn.dgrad(du, kn.pack2(w1)[1], e, addend=g_y)
+    gw1 = _f32(ff, e, device=dev)
+    kn.wgrad(x, du, gw1)
+    return g_x, (gw1, gb1, gw2, gb2, gg, gbe)
 
 
 class _EncoderLayerFn(torch.autograd.Function):
-    """forward_post (detr_backbone.py:157-170) with everything the backward needs kept in bf16; backward = the chain
-    LayerNorm2 <- linear2 (+ReLU mask, fused) <- linear1 <- LayerNorm1 <- out_proj <- attention core <- in_proj on the H100 kernels"""
+    """forward_post (detr_backbone.py:157-170) = attention block + FFN block, with everything the backward needs kept in bf16"""
 
     NAMES = ("self_attn.in_proj_weight", "self_attn.in_proj_bias", "self_attn.out_proj.weight", "self_attn.out_proj.bias", "linear1.weight", "linear1.bias",
              "linear2.weight", "linear2.bias", "norm1.weight", "norm1.bias", "norm2.weight", "norm2.bias")
+    PARAMS = operator.attrgetter(*NAMES)  # layer -> its parameters in NAMES order
+
+    @staticmethod
+    def run(layer, src, pos, mask, params, drop, save):
+        """drop = (p, 4 seeds): attention probabilities, dropout1, FFN dropout, dropout2"""
+        kn = layer.k
+        w_in, b_in, w_o, b_o, w1, b1, w2, b2, g1, be1, g2, be2 = params
+        pd, sd = drop
+        x = _bl(src)
+        qk = x if pos is None else kn.add(x, _bl(pos))
+        x1, s_att = _attention_fwd(kn, layer.nhead, x, qk, None, mask, (w_in, b_in, w_o, b_o, g1, be1), pd, sd[0:2], save)
+        out, s_ffn = _ffn_fwd(kn, x1, (w1, b1, w2, b2, g2, be2), pd, sd[2:4], save)
+        return _lb(out), (s_att, s_ffn)
 
     @staticmethod
     def forward(ctx, layer, src, pos, mask, *params):
-        kn, e, heads = layer.k, layer.d_model, layer.nhead
-        w_in, b_in, w_o, b_o, w1, b1, w2, b2, g1, be1, g2, be2 = params
-        x = _bl(src)
-        qk = x if pos is None else kn.add(x, _bl(pos))
-        b, _, l, _ = x.shape
-        qkv = torch.empty(b, 1, l, 3 * e, dtype=torch.bfloat16, device=x.device)
-        kn.linear(qk, w_in[:2 * e], b_in[:2 * e], out=qkv, out_off=0)
-        kn.linear(x, w_in[2 * e:], b_in[2 * e:], out=qkv, out_off=2 * e)
-        pd, sd = layer._dropout_state(4)  # (p, seeds): attention probabilities, dropout1, FFN dropout, dropout2 (detr_backbone.py:157-170)
-        att, lse = kn.attention_train((qkv, 0, e), (qkv, e, e), (qkv, 2 * e, e), mask, heads, pd, sd[0])
-        if pd > 0:
-            y1 = kn.dropout(kn.linear(att, w_o, b_o), pd, sd[1], residual=x)
-        else:
-            y1 = kn.linear(att, w_o, b_o, residual=x)
-        x1, st1 = kn.layernorm_train(y1, g1, be1)
-        h = kn.linear(x1, w1, b1, relu=True)
-        if pd > 0:
-            h = kn.dropout(h, pd, sd[2])  # the dropped activation is what linear2 sees and what the backward needs (h > 0 and kept)
-            y2 = kn.dropout(kn.linear(h, w2, b2), pd, sd[3], residual=x1)
-        else:
-            y2 = kn.linear(h, w2, b2, residual=x1)
-        out, st2 = kn.layernorm_train(y2, g2, be2)
-        ctx.drop = (pd, sd)
-        ctx.layer, ctx.mask, ctx.has_pos = layer, mask, pos is not None
-        ctx.saved = (x, qk, qkv, att, lse, y1, st1, x1, h, y2, st2)
-        ctx.params = params
-        return _lb(out)
+        out, ctx.saved = _EncoderLayerFn.run(layer, src, pos, mask, params, layer._dropout_state(4), True)
+        ctx.layer, ctx.has_pos = layer, pos is not None
+        return out
 
     @staticmethod
     def backward(ctx, g_out):
-        layer = ctx.layer
-        kn, e, heads = layer.k, layer.d_model, layer.nhead
-        x, qk, qkv, att, lse, y1, st1, x1, h, y2, st2 = ctx.saved
-        w_in, b_in, w_o, b_o, w1, b1, w2, b2, g1, be1, g2, be2 = ctx.params
-        dev = x.device
-        ff = w1.shape[0]
-        g = _bl(g_out)
-        # LayerNorm 2
-        pd, sd = ctx.drop
-        g_y2, gg2, gb2 = kn.layernorm_bwd(g, y2, st2, g2)
-        # linear2 (+ residual to x1) and the ReLU in front of it; with dropout: g_t = dropout2's mask on the branch gradient, and the saved h is the
-        # dropped activation (positive <=> positive and kept), so the ReLU mask also applies the FFN dropout mask -- its 1 / (1 - p) follows
-        g_t = kn.dropout(g_y2, pd, sd[3]) if pd > 0 else g_y2
-        _, w2d = kn.pack2(w2)
-        du, gb1 = kn.dgrad_relu(g_t, w2d, h)
-        if pd > 0:
-            du = kn.dropout(du, pd, sd[2])
-            gb1 = gb1 / (1.0 - pd)
-        gw2 = torch.empty(e, ff, device=dev)
-        kn.wgrad(h, g_t, gw2)
-        gb2_lin = torch.empty(e, device=dev)
-        kn.colsum(g_t, gb2_lin)
-        # linear1; the residual branch of x1 joins through the addend
-        _, w1d = kn.pack2(w1)
-        g_x1 = kn.dgrad(du, w1d, e, addend=g_y2)
-        gw1 = torch.empty(ff, e, device=dev)
-        kn.wgrad(x1, du, gw1)
-        # LayerNorm 1
-        g_y1, gg1, gb1n = kn.layernorm_bwd(g_x1, y1, st1, g1)
-        # out_proj (+ residual to x)
-        g_o = kn.dropout(g_y1, pd, sd[1]) if pd > 0 else g_y1
-        _, wod = kn.pack2(w_o)
-        g_att = kn.dgrad(g_o, wod, e)
-        gwo = torch.empty(e, e, device=dev)
-        kn.wgrad(att, g_o, gwo)
-        gbo = torch.empty(e, device=dev)
-        kn.colsum(g_o, gbo)
-        # attention core
-        dqkv = torch.empty_like(qkv)
-        kn.attention_bwd((qkv, 0, e), (qkv, e, e), (qkv, 2 * e, e), att, g_att, ctx.mask, heads, lse, (dqkv, 0, e), (dqkv, e, e), (dqkv, 2 * e, e), pd, sd[0])
-        # in_proj: q, k from qk = x + pos; v from x
-        _, wqkd = kn.pack2(w_in[:2 * e])
-        _, wvd = kn.pack2(w_in[2 * e:])
-        g_qk = kn.dgrad((dqkv, 0, 2 * e), wqkd, e)
-        g_x = kn.dgrad((dqkv, 2 * e, e), wvd, e, addend=g_y1)
-        g_src = kn.add(g_x, g_qk)
-        gw_in = torch.empty(3 * e, e, device=dev)
-        kn.wgrad(qk, (dqkv, 0, 2 * e), gw_in[:2 * e])
-        kn.wgrad(x, (dqkv, 2 * e, e), gw_in[2 * e:])
-        gb_in = torch.empty(3 * e, device=dev)
-        kn.colsum(dqkv, gb_in)
-        grads = (gw_in, gb_in, gwo, gbo, gw1, gb1, gw2, gb2_lin, gg1, gb1n, gg2, gb2)
+        kn, heads = ctx.layer.k, ctx.layer.nhead
+        s_att, s_ffn = ctx.saved
+        g_x1, gf = _ffn_bwd(kn, _bl(g_out), s_ffn)
+        g_src, g_qk, _, ga = _attention_bwd(kn, heads, g_x1, s_att)
+        grads = ga[:4] + gf[:4] + ga[4:] + gf[4:]  # NAMES order: projections, then the norms
         return (None, _lb(g_src), _lb(g_qk) if ctx.has_pos else None, None) + grads
 
 
 class _DecoderLayerFn(torch.autograd.Function):
-    """TransformerDecoderLayer.forward_post (detr_backbone.py:221-242) and its backward on the same kernels as `_EncoderLayerFn`:
-    self-attention block, cross-attention block (queries from the decoder stream, keys / values from the encoder memory), FFN block"""
+    """TransformerDecoderLayer.forward_post (detr_backbone.py:221-242) = self-attention block + cross-attention block (queries from the decoder
+    stream, keys / values from the encoder memory) + FFN block, and its backward on the same kernels as `_EncoderLayerFn`"""
 
     NAMES = ("self_attn.in_proj_weight", "self_attn.in_proj_bias", "self_attn.out_proj.weight", "self_attn.out_proj.bias",
              "multihead_attn.in_proj_weight", "multihead_attn.in_proj_bias", "multihead_attn.out_proj.weight", "multihead_attn.out_proj.bias",
              "linear1.weight", "linear1.bias", "linear2.weight", "linear2.bias", "norm1.weight", "norm1.bias", "norm2.weight", "norm2.bias", "norm3.weight", "norm3.bias")
+    PARAMS = operator.attrgetter(*NAMES)
 
     @staticmethod
-    def forward(ctx, layer, tgt, memory, pos, query_pos, tgt_mask, mem_mask, *params):
-        kn, e, heads = layer.k, layer.d_model, layer.nhead
+    def run(layer, tgt, memory, pos, query_pos, tgt_mask, mem_mask, params, drop, save):
+        """drop = (p, 6 seeds): self-attention probabilities, dropout1, cross-attention probabilities, dropout2, FFN dropout, dropout3"""
+        kn, heads = layer.k, layer.nhead
         ws, bs, wso, bso, wc, bc, wco, bco, w1, b1, w2, b2, g1, be1, g2, be2, g3, be3 = params
+        pd, sd = drop
         x = _bl(tgt)
         qp = None if query_pos is None else _bl(query_pos)
         qk = x if qp is None else kn.add(x, qp)
-        b, _, lq, _ = x.shape
-        qkv = torch.empty(b, 1, lq, 3 * e, dtype=torch.bfloat16, device=x.device)
-        kn.linear(qk, ws[:2 * e], bs[:2 * e], out=qkv, out_off=0)
-        kn.linear(x, ws[2 * e:], bs[2 * e:], out=qkv, out_off=2 * e)
-        pd, sd = layer._dropout_state(6)  # self-attention probabilities, dropout1, cross-attention probabilities, dropout2, FFN dropout, dropout3
-        att1, lse1 = kn.attention_train((qkv, 0, e), (qkv, e, e), (qkv, 2 * e, e), tgt_mask, heads, pd, sd[0])
-        y1 = kn.dropout(kn.linear(att1, wso, bso), pd, sd[1], residual=x) if pd > 0 else kn.linear(att1, wso, bso, residual=x)
-        x1, st1 = kn.layernorm_train(y1, g1, be1)
+        x1, s_self = _attention_fwd(kn, heads, x, qk, None, tgt_mask, (ws, bs, wso, bso, g1, be1), pd, sd[0:2], save)
         mem = _bl(memory)
         memk = mem if pos is None else kn.add(mem, _bl(pos))
         q2 = x1 if qp is None else kn.add(x1, qp)
-        qc = kn.linear(q2, wc[:e], bc[:e])
-        lk = mem.shape[2]
-        kv = torch.empty(b, 1, lk, 2 * e, dtype=torch.bfloat16, device=x.device)
-        kn.linear(memk, wc[e:2 * e], bc[e:2 * e], out=kv, out_off=0)
-        kn.linear(mem, wc[2 * e:], bc[2 * e:], out=kv, out_off=e)
-        att2, lse2 = kn.attention_train((qc, 0, e), (kv, 0, e), (kv, e, e), mem_mask, heads, pd, sd[2])
-        y2 = kn.dropout(kn.linear(att2, wco, bco), pd, sd[3], residual=x1) if pd > 0 else kn.linear(att2, wco, bco, residual=x1)
-        x2, st2 = kn.layernorm_train(y2, g2, be2)
-        h = kn.linear(x2, w1, b1, relu=True)
-        if pd > 0:
-            h = kn.dropout(h, pd, sd[4])
-            y3 = kn.dropout(kn.linear(h, w2, b2), pd, sd[5], residual=x2)
-        else:
-            y3 = kn.linear(h, w2, b2, residual=x2)
-        out, st3 = kn.layernorm_train(y3, g3, be3)
-        ctx.drop = (pd, sd)
-        ctx.layer, ctx.masks, ctx.has = layer, (tgt_mask, mem_mask), (pos is not None, query_pos is not None)
-        ctx.saved = (x, qk, qkv, att1, lse1, y1, st1, x1, mem, memk, q2, qc, kv, att2, lse2, y2, st2, x2, h, y3, st3)
-        ctx.params = params
-        return _lb(out)
+        x2, s_cross = _attention_fwd(kn, heads, x1, q2, (memk, mem), mem_mask, (wc, bc, wco, bco, g2, be2), pd, sd[2:4], save)
+        out, s_ffn = _ffn_fwd(kn, x2, (w1, b1, w2, b2, g3, be3), pd, sd[4:6], save)
+        return _lb(out), (s_self, s_cross, s_ffn)
+
+    @staticmethod
+    def forward(ctx, layer, tgt, memory, pos, query_pos, tgt_mask, mem_mask, *params):
+        out, ctx.saved = _DecoderLayerFn.run(layer, tgt, memory, pos, query_pos, tgt_mask, mem_mask, params, layer._dropout_state(6), True)
+        ctx.layer, ctx.has = layer, (pos is not None, query_pos is not None)
+        return out
 
     @staticmethod
     def backward(ctx, g_out):
-        layer = ctx.layer
-        kn, e, heads = layer.k, layer.d_model, layer.nhead
-        x, qk, qkv, att1, lse1, y1, st1, x1, mem, memk, q2, qc, kv, att2, lse2, y2, st2, x2, h, y3, st3 = ctx.saved
-        ws, bs, wso, bso, wc, bc, wco, bco, w1, b1, w2, b2, g1, be1, g2, be2, g3, be3 = ctx.params
-        tgt_mask, mem_mask = ctx.masks
+        kn, heads = ctx.layer.k, ctx.layer.nhead
+        s_self, s_cross, s_ffn = ctx.saved
         has_pos, has_qpos = ctx.has
-        dev, ff = x.device, w1.shape[0]
-        f32 = lambda *shape: torch.empty(*shape, device=dev)
-        g = _bl(g_out)
-        # FFN block
-        pd, sd = ctx.drop
-        g_y3, gg3, gbn3 = kn.layernorm_bwd(g, y3, st3, g3)
-        g_t = kn.dropout(g_y3, pd, sd[5]) if pd > 0 else g_y3
-        du, gb1 = kn.dgrad_relu(g_t, kn.pack2(w2)[1], h)
-        if pd > 0:
-            du = kn.dropout(du, pd, sd[4])
-            gb1 = gb1 / (1.0 - pd)
-        gw2, gb2 = f32(e, ff), f32(e)
-        kn.wgrad(h, g_t, gw2)
-        kn.colsum(g_t, gb2)
-        g_x2 = kn.dgrad(du, kn.pack2(w1)[1], e, addend=g_y3)
-        gw1 = f32(ff, e)
-        kn.wgrad(x2, du, gw1)
-        # cross-attention block
-        g_y2, gg2, gbn2 = kn.layernorm_bwd(g_x2, y2, st2, g2)
-        g_o2 = kn.dropout(g_y2, pd, sd[3]) if pd > 0 else g_y2
-        g_att2 = kn.dgrad(g_o2, kn.pack2(wco)[1], e)
-        gwco, gbco = f32(e, e), f32(e)
-        kn.wgrad(att2, g_o2, gwco)
-        kn.colsum(g_o2, gbco)
-        dqc, dkv = torch.empty_like(qc), torch.empty_like(kv)
-        kn.attention_bwd((qc, 0, e), (kv, 0, e), (kv, e, e), att2, g_att2, mem_mask, heads, lse2, (dqc, 0, e), (dkv, 0, e), (dkv, e, e), pd, sd[2])
-        g_q2 = kn.dgrad(dqc, kn.pack2(wc[:e])[1], e)
-        g_memk = kn.dgrad((dkv, 0, e), kn.pack2(wc[e:2 * e])[1], e)
-        g_mem = kn.dgrad((dkv, e, e), kn.pack2(wc[2 * e:])[1], e, addend=g_memk)  # memory feeds keys (through + pos) and values
-        gwc, gbc = f32(3 * e, e), f32(3 * e)
-        kn.wgrad(q2, dqc, gwc[:e])
-        kn.wgrad(memk, (dkv, 0, e), gwc[e:2 * e])
-        kn.wgrad(mem, (dkv, e, e), gwc[2 * e:])
-        kn.colsum(dqc, gbc[:e])
-        kn.colsum(dkv, gbc[e:])
-        g_x1 = kn.add(g_y2, g_q2)  # residual branch + query path
-        # self-attention block
-        g_y1, gg1, gbn1 = kn.layernorm_bwd(g_x1, y1, st1, g1)
-        g_o1 = kn.dropout(g_y1, pd, sd[1]) if pd > 0 else g_y1
-        g_att1 = kn.dgrad(g_o1, kn.pack2(wso)[1], e)
-        gwso, gbso = f32(e, e), f32(e)
-        kn.wgrad(att1, g_o1, gwso)
-        kn.colsum(g_o1, gbso)
-        dqkv = torch.empty_like(qkv)
-        kn.attention_bwd((qkv, 0, e), (qkv, e, e), (qkv, 2 * e, e), att1, g_att1, tgt_mask, heads, lse1, (dqkv, 0, e), (dqkv, e, e), (dqkv, 2 * e, e), pd, sd[0])
-        g_qk = kn.dgrad((dqkv, 0, 2 * e), kn.pack2(ws[:2 * e])[1], e)
-        g_x = kn.dgrad((dqkv, 2 * e, e), kn.pack2(ws[2 * e:])[1], e, addend=g_y1)
-        g_tgt = kn.add(g_x, g_qk)
-        gws, gbs = f32(3 * e, e), f32(3 * e)
-        kn.wgrad(qk, (dqkv, 0, 2 * e), gws[:2 * e])
-        kn.wgrad(x, (dqkv, 2 * e, e), gws[2 * e:])
-        kn.colsum(dqkv, gbs)
+        g_x2, gf = _ffn_bwd(kn, _bl(g_out), s_ffn)
+        g_x1, g_q2, (g_mem, g_memk), gc = _attention_bwd(kn, heads, g_x2, s_cross)
+        g_tgt, g_qk, _, gs = _attention_bwd(kn, heads, g_x1, s_self)
         g_qpos = _lb(kn.add(g_qk, g_q2)) if has_qpos else None
-        grads = (gws, gbs, gwso, gbso, gwc, gbc, gwco, gbco, gw1, gb1, gw2, gb2, gg1, gbn1, gg2, gbn2, gg3, gbn3)
+        grads = gs[:4] + gc[:4] + gf[:4] + gs[4:] + gc[4:] + gf[4:]  # NAMES order: projections, then the norms
         return (None, _lb(g_tgt), _lb(g_mem), _lb(g_memk) if has_pos else None, g_qpos, None, None) + grads
 
 
@@ -502,22 +471,12 @@ class TransformerEncoderLayer(_LayerBase):
     def forward(self, src, src_mask=None, src_key_padding_mask=None, pos=None):
         if src_mask is not None:
             raise capi.Yb200Error("attn_mask is not supported (the reference's DETR never passes one)")
-        if not src.is_cuda:
-            raise capi.Yb200Error("DETR layers: inputs must be CUDA tensors (no CPU path)")
-        if TRAINING_PATH and torch.is_grad_enabled():
-            params = [dict(self.named_parameters())[n] for n in _EncoderLayerFn.NAMES]
-            if src.requires_grad or any(p.requires_grad for p in params):
-                return _EncoderLayerFn.apply(self, src, pos, _mask_u8(src_key_padding_mask), *params)
-        with torch.no_grad():
-            return self._forward_inference(src, src_key_padding_mask, pos)
-
-    def _forward_inference(self, src, src_key_padding_mask, pos):
-        _check_inputs(src, pos)
-        x = _bl(src)
-        qk = x if pos is None else self.k.add(x, _bl(pos))
-        y = self._self_attention(x, qk, self.self_attn, _mask_u8(src_key_padding_mask))
-        x1 = self.k.layernorm(y, self.norm1.weight, self.norm1.bias)
-        return _lb(self._ffn(x1, self.norm2))
+        _check_devices(src, pos, src_key_padding_mask)
+        params = _EncoderLayerFn.PARAMS(self)
+        mask = _mask_u8(src_key_padding_mask)
+        if _records(src, *params):
+            return _EncoderLayerFn.apply(self, src, pos, mask, *params)
+        return _EncoderLayerFn.run(self, src, pos, mask, params, _NO_DROPOUT, False)[0]
 
 
 class TransformerDecoderLayer(_LayerBase):
@@ -532,33 +491,12 @@ class TransformerDecoderLayer(_LayerBase):
     def forward(self, tgt, memory, tgt_mask=None, memory_mask=None, tgt_key_padding_mask=None, memory_key_padding_mask=None, pos=None, query_pos=None):
         if tgt_mask is not None or memory_mask is not None:
             raise capi.Yb200Error("attn_mask is not supported (the reference's DETR never passes one)")
-        if TRAINING_PATH and torch.is_grad_enabled():
-            params = [dict(self.named_parameters())[n] for n in _DecoderLayerFn.NAMES]
-            if tgt.requires_grad or memory.requires_grad or any(p.requires_grad for p in params):
-                return _DecoderLayerFn.apply(self, tgt, memory, pos, query_pos, _mask_u8(tgt_key_padding_mask), _mask_u8(memory_key_padding_mask), *params)
-        with torch.no_grad():
-            return self._forward_inference(tgt, memory, tgt_key_padding_mask, memory_key_padding_mask, pos, query_pos)
-
-    def _forward_inference(self, tgt, memory, tgt_key_padding_mask, memory_key_padding_mask, pos, query_pos):
-        _check_inputs(tgt, memory, pos, query_pos)
-        kn, e = self.k, self.d_model
-        x = _bl(tgt)
-        qp = None if query_pos is None else _bl(query_pos)
-        qk = x if qp is None else kn.add(x, qp)
-        x = kn.layernorm(self._self_attention(x, qk, self.self_attn, _mask_u8(tgt_key_padding_mask)), self.norm1.weight, self.norm1.bias)
-        # cross attention: queries from the decoder stream, keys / values from the encoder memory
-        mem = _bl(memory)
-        memk = mem if pos is None else kn.add(mem, _bl(pos))
-        att = self.multihead_attn
-        w, bias = att.in_proj_weight, att.in_proj_bias
-        q = kn.linear(x if qp is None else kn.add(x, qp), w[:e], bias[:e])
-        b, _, lk, _ = mem.shape
-        kv = torch.empty(b, 1, lk, 2 * e, dtype=torch.bfloat16, device=mem.device)
-        kn.linear(memk, w[e:2 * e], bias[e:2 * e], out=kv, out_off=0)
-        kn.linear(mem, w[2 * e:], bias[2 * e:], out=kv, out_off=e)
-        a = kn.attention((q, 0, e), (kv, 0, e), (kv, e, e), _mask_u8(memory_key_padding_mask), self.nhead)
-        x = kn.layernorm(kn.linear(a, att.out_proj.weight, att.out_proj.bias, residual=x), self.norm2.weight, self.norm2.bias)
-        return _lb(self._ffn(x, self.norm3))
+        _check_devices(tgt, memory, pos, query_pos, tgt_key_padding_mask, memory_key_padding_mask)
+        params = _DecoderLayerFn.PARAMS(self)
+        masks = _mask_u8(tgt_key_padding_mask), _mask_u8(memory_key_padding_mask)
+        if _records(tgt, memory, *params):
+            return _DecoderLayerFn.apply(self, tgt, memory, pos, query_pos, *masks, *params)
+        return _DecoderLayerFn.run(self, tgt, memory, pos, query_pos, *masks, params, _NO_DROPOUT, False)[0]
 
 
 # ------------------------------------------------------------------------------------------------------------------------------------
@@ -594,10 +532,9 @@ class LayerNorm(nn.Module):
     def forward(self, x):
         if not x.is_cuda:
             raise capi.Yb200Error("DETR layers: inputs must be CUDA tensors (no CPU path)")
-        if TRAINING_PATH and torch.is_grad_enabled() and (x.requires_grad or self.weight.requires_grad):
+        if _records(x, self.weight):
             return _LayerNormFn.apply(self.k, x, self.weight, self.bias)
-        with torch.no_grad():
-            return _lb(self.k.layernorm(_bl(x), self.weight, self.bias))
+        return _lb(self.k.layernorm(_bl(x), self.weight, self.bias)[0])
 
 
 def _clone_layer(layer):
@@ -710,22 +647,12 @@ class _LinearStackFn(torch.autograd.Function):
         hs, wds = [h], []
         for i, (w, b) in enumerate(zip(ws, bs)):
             last = i == len(ws) - 1
-            cout, cpad = w.shape[0], _pad16(w.shape[0])
-            wf = torch.empty(cpad, 1, w.shape[1], dtype=torch.bfloat16, device=x.device)
-            wd = torch.empty(w.shape[1], 1, cpad, dtype=torch.bfloat16, device=x.device)
-            capi.check(kn.L.yb200_pack_conv_weight(capi.ptr(w.detach().contiguous()), cout, w.shape[1], 1, cpad, w.shape[1], capi.ptr(wf), capi.ptr(wd),
-                                                   capi.stream_ptr()), "pack")
+            cpad = _pad16(w.shape[0])
+            wf, wd = kn.pack2(w, cpad)
             bias = torch.zeros(cpad, device=x.device)
-            bias[:cout] = b.detach()
-            out = torch.empty(1, 1, n, cpad, dtype=torch.bfloat16, device=x.device)
-            ha, oa = kn._a(h), kn._a(out)
-            if last:
-                capi.check(kn.L.yb200_conv2d_affine_fwd(ctypes.byref(ha), capi.ptr(wf), None, capi.ptr(bias), None, ctypes.byref(oa), 1, 1, capi.stream_ptr()),
-                           "linear")
-            else:
-                capi.check(kn.L.yb200_linear_relu_fwd(ctypes.byref(ha), capi.ptr(wf), capi.ptr(bias), ctypes.byref(oa), capi.stream_ptr()), "linear+relu")
+            bias[:w.shape[0]] = b.detach()
+            h = kn.linear(h, wf, bias, relu=not last)
             wds.append(wd)
-            h = out
             if not last:
                 hs.append(h)
         ctx.kn, ctx.hs, ctx.wds, ctx.couts, ctx.lead, ctx.cin = kn, hs, wds, [w.shape[0] for w in ws], lead, cin

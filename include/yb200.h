@@ -287,7 +287,8 @@ int yb200_conv2d_affine_fwd(const yb200_act* x, const void* w_fwd, const float* 
                             const yb200_act* out, int ksize, int stride, void* stream);
 /* pwconv1 + GELU (convnext.py:52-53): u = bf16(x W^T + bias) -> u_out (may be NULL), h = bf16(GELU(u)) -> h_out (exact erf form)       */
 int yb200_linear_gelu_fwd(const yb200_act* x, const void* w_fwd, const float* bias, const yb200_act* u_out, const yb200_act* h_out, void* stream);
-/* du = bf16((dz W) * GELU'(u)) and, when bias_grad_sum != NULL, bias_grad_sum[c] += sum over pixels of du[.., c] (fp64, caller zeroes it):
+/* du = bf16((dz W) * GELU'(u)) and, when bias_grad_sum != NULL, bias_grad_sum[c] += sum over pixels of the stored bf16 du[.., c] (fp32 per
+ * CTA, then fp64 atomics into the caller's accumulator):
  * the data gradient of pwconv2 fused with the GELU backward and the bias gradient of pwconv1.                                            */
 int yb200_linear_dgrad_gelu(const yb200_act* dz, const void* w_dgrad, const yb200_act* u, const yb200_act* du, double* bias_grad_sum,
                             void* stream);
@@ -332,7 +333,9 @@ int yb200_attention_fwd(const yb200_act* q, const yb200_act* k, const yb200_act*
                         const yb200_act* out, float* lse, void* stream);
 /* Linear + ReLU of the transformer FFN (detr_backbone.py:167, 239): h = bf16(max(x W^T + bias, 0))                                        */
 int yb200_linear_relu_fwd(const yb200_act* x, const void* w_fwd, const float* bias, const yb200_act* h_out, void* stream);
-/* du = bf16(h > 0 ? dz W : 0) and optionally bias_grad_sum[c] += column sums of du (fp64): data gradient of linear2 fused with ReLU backward */
+/* du = bf16(h > 0 ? dz W : 0) (h > 0: positive and non-zero; -0 and negatives mask) and optionally bias_grad_sum[c] += column sums of the
+ * STORED bf16 du (summed in fp32 inside each CTA, added to the caller's fp64 accumulator with one atomic per CTA and column: the order of
+ * those additions is not fixed): data gradient of linear2 fused with the ReLU backward and the bias gradient of linear1               */
 int yb200_linear_dgrad_relu(const yb200_act* dz, const void* w_dgrad, const yb200_act* h, const yb200_act* du, double* bias_grad_sum, void* stream);
 /* out = a + b (bf16 views of equal shape): tensor + positional embedding (detr_backbone.py:154-155, 218-219)                                */
 int yb200_add(const yb200_act* a, const yb200_act* b, const yb200_act* out, void* stream);

@@ -38,23 +38,25 @@ def _thr24(p):
     return int(float(torch.tensor(p, dtype=torch.float32)) * 16777216.0)
 
 
-def dropout_multiplier(seed, shape_blc, p):
-    """[B, L, C] multiplier (0 or 1/(1-p)) of yb200_dropout for a [B][1][L][C] activation: element index ((b*L + l)*C + c)"""
+def dropout_multiplier(seed, shape_blc, p, device=None):
+    """[B, L, C] multiplier (0 or 1/(1-p)) of yb200_dropout for a [B][1][L][C] activation: element index ((b*L + l)*C + c).  device: where
+    to evaluate the hash (default: the CPU)"""
     n = 1
     for d in shape_blc:
         n *= d
-    e = torch.arange(n, dtype=torch.int64)
+    e = torch.arange(n, dtype=torch.int64, device=device)
     keep = (_mix32(seed ^ ((e * 0x9E3779B1) & _M)) >> 8) >= _thr24(p)
     inv = float(torch.tensor(1.0, dtype=torch.float32) / (torch.tensor(1.0, dtype=torch.float32) - torch.tensor(p, dtype=torch.float32)))
     return (keep.to(torch.float32) * inv).view(*shape_blc)
 
 
-def attention_dropout_multiplier(seed, b, heads, lq, lk, p):
-    """[B, H, Lq, Lk] multiplier of yb200_attention_fwd_dropout: row key from (seed, b*H + h, q), element from the key index"""
-    bh = torch.arange(b * heads, dtype=torch.int64)[:, None]
-    q = torch.arange(lq, dtype=torch.int64)[None, :]
+def attention_dropout_multiplier(seed, b, heads, lq, lk, p, device=None):
+    """[B, H, Lq, Lk] multiplier of yb200_attention_fwd_dropout: row key from (seed, b*H + h, q), element from the key index.  device: where
+    to evaluate the hash (default: the CPU; B = 16 at 1050 x 1050 tokens is 141 M elements)"""
+    bh = torch.arange(b * heads, dtype=torch.int64, device=device)[:, None]
+    q = torch.arange(lq, dtype=torch.int64, device=device)[None, :]
     row = _mix32(seed ^ _mix32((bh * 0x9E3779B1 + q + 0x7F4A7C15) & _M))
-    col = (torch.arange(lk, dtype=torch.int64) * 0x9E3779B1) & _M
+    col = (torch.arange(lk, dtype=torch.int64, device=device) * 0x9E3779B1) & _M
     keep = (_mix32(row[..., None] ^ col) >> 8) >= _thr24(p)
     inv = float(torch.tensor(1.0, dtype=torch.float32) / (torch.tensor(1.0, dtype=torch.float32) - torch.tensor(p, dtype=torch.float32)))
     return (keep.to(torch.float32) * inv).view(b, heads, lq, lk)

@@ -359,6 +359,31 @@ int yb200_sigmoid(const yb200_act* x, const yb200_act* out, void* stream);
 /* inst[r][c] = raw[r][c] / max(normalizer[r], 1e-6) -> bf16 [1][1][rows][cols] view (:75-76).  raw = iam_prob^T features of one image is
  * yb200_conv2d_wgrad(x = features, dz = iam_prob, ksize 1) (the pixel contraction of :74), normalizer = yb200_colsum(iam_prob).              */
 int yb200_iam_normalize(const float* raw, const float* normalizer, int rows, int cols, const yb200_act* out, void* stream);
+
+/* ---- SparseInst IAM decoder backward (decoder_sparseinst.py:27-250) -------------------------------------------------------------------------
+ * Fixed summation order and no atomics in every call below: bit-reproducible.
+ * yb200_conv2d_dgrad_relu: dx = bf16((h > 0 ? dz W : 0) + addend) -- the data gradient of a convolution whose input h is a ReLU output
+ *   (`_make_stack_3x3_convs` :18-24), masked before addend (may be NULL) is added: pass an addend that is already masked.  ksize 1 or 3,
+ *   stride 1; h and dx have the same shape and channel pitch.
+ * yb200_upsample_bilinear2x_bwd_f32: the adjoint of yb200_upsample_bilinear2x_f32 (:148-153): dout fp32 [dx->n][maps][2h][2w] -> dx bf16
+ *   [n][h][w][c] view (maps <= c; channels >= maps written as 0), the NHWC operand of the mask GEMM's gradients.  Each element sums its
+ *   (up to 16) up-sampled contributions.
+ * yb200_iam_normalize_bwd: backward of yb200_iam_normalize for a batch (:75-76, group :225-235).  g: bf16 [n][1][R][(rows / rows_per_group) *
+ *   cols] view, the gradient of inst; raw row r reads row r % rows_per_group, columns from (r / rows_per_group) * cols (the grouped decoder's
+ *   reshape(B, G, N, C).transpose(1, 2); rows of r % rows_per_group >= R read as 0).  raw fp32 [n][rows][cols], normalizer fp32 [n][rows].
+ *   Writes d raw = g / max(normalizer, 1e-6) as bf16 draw [n][rows][cols] and draw_t [n][cols][rows], and dnorm fp32 [n][rows] =
+ *   -sum_c draw raw / max(normalizer, 1e-6) (= -sum_c g raw / max(normalizer, 1e-6)^2, summed from the stored bf16 d raw so that the
+ *   normalisation's invariance to a common scale of the probabilities holds for the operands the aggregation backward reads; 0 where
+ *   normalizer < 1e-6, the clamp).  cols <= 2048.
+ * yb200_sigmoid_bwd: dx = dy * sigmoid'(x) with sigmoid' recomputed in fp32 from x (:67), the channels regrouped: dx channel
+ *   k * group_out + i = (i < group_in ? dy * sigmoid'(x) at channel k * group_in + i : 0).  dy and x have the same shape; dx the same
+ *   pixels and dy->c / group_in * group_out channels; group_in, group_out multiples of 8.                                                       */
+int yb200_conv2d_dgrad_relu(const yb200_act* dz, const void* w_dgrad, const yb200_act* h, const yb200_act* dx, const yb200_act* addend, int ksize,
+                            int stride, void* stream);
+int yb200_upsample_bilinear2x_bwd_f32(const float* dout, int maps, const yb200_act* dx, void* stream);
+int yb200_iam_normalize_bwd(const yb200_act* g, const float* raw, const float* normalizer, int rows, int cols, int rows_per_group, void* draw,
+                            void* draw_t, float* dnorm, void* stream);
+int yb200_sigmoid_bwd(const yb200_act* dy, const yb200_act* x, const yb200_act* dx, int group_in, int group_out, void* stream);
 /* Backward of yb200_attention_fwd: given out, its gradient dout and the saved lse, dq / dk / dv (bf16 views shaped like q / k / k; they may be
  * slices of one packed buffer).  P is recomputed from lse; two kernels (per key tile: dK, dV; per query tile: dQ), accumulation in registers,
  * no atomics.  workspace: yb200_attention_bwd_workspace(q) bytes (D = <dout, out> per query row and head).                                     */

@@ -650,6 +650,16 @@ extern "C" int yb200_linear_dgrad_relu(const yb200_act* dz, const void* w_dgrad,
   return dgrad_impl(dz, w_dgrad, du, nullptr, 1, 1, h, bias_grad_sum, stream, EPI_BF16_RELU_BWD);
 }
 
+extern "C" int yb200_conv2d_dgrad_relu(const yb200_act* dz, const void* w_dgrad, const yb200_act* h, const yb200_act* dx, const yb200_act* addend,
+                                       int ksize, int stride, void* stream) {
+  int rc;
+  if ((rc = check_arg(h, "conv2d_dgrad_relu", "h"))) return rc;
+  if ((rc = check_arg(dx, "conv2d_dgrad_relu", "dx"))) return rc;
+  YB_REQUIRE((ksize == 1 || ksize == 3) && stride == 1, YB200_ERR_UNSUPPORTED, "conv2d_dgrad_relu: ksize=%d stride=%d not implemented", ksize, stride);
+  YB_REQUIRE(same_geometry(h, dx), YB200_ERR_INVALID, "conv2d_dgrad_relu: h and dx must have the same shape and channel pitch");
+  return dgrad_impl(dz, w_dgrad, dx, addend, ksize, stride, h, nullptr, stream, EPI_BF16_RELU_BWD);
+}
+
 // ------------------------------------------------------------------------------------------------
 // weight gradient
 // ------------------------------------------------------------------------------------------------

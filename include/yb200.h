@@ -489,6 +489,29 @@ int yb200_sparseinst_set_loss_bwd(const float* logits, const float* masks, const
                                   int num_pairs, float w_ce, float w_obj, float w_dice, float w_mask, float num_instances, const float* grad,
                                   float* dlogits, float* dmasks, float* dscores, void* stream);
 
+/* ---- SparseInst InstanceContextEncoder (yolov7/modeling/transcoders/encoder_sparseinst.py:18-127) -----------------------------------------
+ * The non-GEMM steps of the encoder and their adjoints, on NHWC bf16 views (channel slices of the concat buffers).  The convolutions are
+ * yb200_conv2d_affine_fwd / yb200_conv2d_relu_fwd, their gradients yb200_conv2d_dgrad[_relu], yb200_conv2d_wgrad and yb200_colsum.  Every sum
+ * runs in fp32 in a fixed order, rounded to bf16 once; no atomics: bit-reproducible.
+ *   yb200_avg_pool2d: MyAdaptiveAvgPool2d (:18-39), which is F.avg_pool2d with kernel = stride = (kh, kw) = (ceil(H/s), ceil(W/s)), floor
+ *     mode, no padding: out [n][h/kh][w/kw][c] = window sum / (kh * kw).
+ *   yb200_ppm_input_grad: the gradient of the PPM's input (:56-68): dx = dcat + sum over the stages i < nstages, in order, of the adjoint of
+ *     the pool, dpooled[i] / (kh * kw) at every pixel of the window that covers it (pixels beyond the last full window get dcat only).
+ *     dpooled: HOST array of nstages (<= 8) views, each [dx->n][dx->h / kh][dx->w / kw][dx->c]; kernel_hw: HOST int32 [nstages][2] = (kh, kw).
+ *   yb200_resize_bilinear: F.interpolate(x, size=(out->h, out->w), mode="bilinear", align_corners=False) (:58-66, :121-125) with ATen's index
+ *     arithmetic: scale = in / out, src = max(scale * (dst + 0.5) - 0.5, 0), i1 = i0 + (i0 < in - 1), fp32 weights.
+ *   yb200_resize_bilinear_bwd: its adjoint, dx (the input's shape) = for every input pixel the weighted sum of the d out pixels whose taps
+ *     reach it; h (may be NULL, dx's shape): dx = h > 0 ? sum : 0, the gradient of z in interpolate(relu(z)).
+ *   yb200_upsample_nearest2x_add: the top-down path (:114-118), out = lat + F.interpolate(coarse, scale_factor=2, mode="nearest"); out may
+ *     be lat.
+ *   yb200_upsample_nearest2x_bwd: its adjoint, dx [n][h/2][w/2][c] = the 2x2 sums of dy; h (may be NULL, dx's shape): dx = h > 0 ? sum : 0. */
+int yb200_avg_pool2d(const yb200_act* x, int kh, int kw, const yb200_act* out, void* stream);
+int yb200_ppm_input_grad(const yb200_act* dcat, const yb200_act* dpooled, const int32_t* kernel_hw, int nstages, const yb200_act* dx, void* stream);
+int yb200_resize_bilinear(const yb200_act* x, const yb200_act* out, void* stream);
+int yb200_resize_bilinear_bwd(const yb200_act* dout, const yb200_act* h, const yb200_act* dx, void* stream);
+int yb200_upsample_nearest2x_add(const yb200_act* lat, const yb200_act* coarse, const yb200_act* out, void* stream);
+int yb200_upsample_nearest2x_bwd(const yb200_act* dy, const yb200_act* h, const yb200_act* dx, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -3,7 +3,7 @@
 # usage: tools/gpu_suite.sh [group ...]   logs -> profile_out/suite_<group>.log
 mkdir -p profile_out
 groups=("$@")
-[ ${#groups[@]} -eq 0 ] && groups=(conv_fwd fwd_b fwd_c fwd_d fwd_e conv_misc conv_dgrad conv_wgrad elementwise simota nms engine modeling iou fused optim streams fixed_order train_bn mosaic cnx_ops cnx_engine attention detr detr_dropout sparseinst strict yolox_convnext detr_criterion convnext_plan sparseinst_kernels sparseinst_criterion detr_kernels sparseinst_bwd)
+[ ${#groups[@]} -eq 0 ] && groups=(conv_fwd fwd_b fwd_c fwd_d fwd_e conv_misc conv_dgrad conv_wgrad elementwise simota nms engine modeling iou fused optim streams fixed_order train_bn mosaic cnx_ops cnx_engine attention detr detr_dropout sparseinst strict yolox_convnext detr_criterion convnext_plan sparseinst_kernels sparseinst_criterion detr_kernels sparseinst_bwd sparseinst_encoder)
 for g in "${groups[@]}"; do
   case $g in
     conv_fwd)    sel="tests/test_conv_gpu.py -k 'test_conv_fwd_stats and not 1x320 and not 16x64 and not 8x80x80'" ;;
@@ -38,6 +38,7 @@ for g in "${groups[@]}"; do
     sparseinst_kernels) sel="tests/test_sparseinst_kernels_gpu.py" ;;
     sparseinst_criterion) sel="tests/test_sparseinst_criterion_gpu.py" ;;
     sparseinst_bwd) sel="tests/test_sparseinst_bwd_gpu.py" ;;
+    sparseinst_encoder) sel="tests/test_sparseinst_encoder_gpu.py" ;;
     detr_kernels) sel="tests/test_detr_kernels_gpu.py" ;;
     cnx_ops)     sel="tests/test_convnext_gpu.py -k 'not engine and not block_against'" ;;
     cnx_engine)  sel="tests/test_convnext_gpu.py -k 'engine or block_against'" ;;

@@ -55,20 +55,28 @@ def bound(ref, mag, k, r_store, inner=None, r_inner=0.0):
     return b
 
 
+SLAB = 1 << 25  # elements compared per step: the fp64 temporaries of a check stay ~1 GB at the 64 x 640 x 640 plan's sizes
+
+
 def excess(got, ref, bnd):
     """worst |got - ref| / bound over the elements (inf if any value is not finite)"""
-    got = got.double()
-    if not torch.isfinite(got).all():
-        return math.inf
-    return float(((got - ref).abs() / bnd.clamp_min(1e-300)).max())
+    got, ref, bnd = got.reshape(-1), ref.reshape(-1), bnd.reshape(-1)
+    worst = 0.0
+    for i in range(0, got.numel(), SLAB):
+        sl = slice(i, i + SLAB)
+        gs = got[sl].double()
+        if not torch.isfinite(gs).all():
+            return math.inf
+        worst = max(worst, float(((gs - ref[sl]).abs() / bnd[sl].clamp_min(1e-300)).max()))
+    return worst
 
 
 def check(cls, got, ref, bnd, what):
-    got = got.double()
     r = excess(got, ref, bnd)
     WORST[cls] = max(WORST.get(cls, 0.0), r)
     if r <= 1.0:
         return
+    got = got.double()
     if not torch.isfinite(got).all():
         bad = (~torch.isfinite(got)).nonzero()
         raise AssertionError(f"{what}: {bad.shape[0]} non-finite values, first at {bad[0].tolist()}")
@@ -92,48 +100,62 @@ def _pad(x, p):
     return F.pad(x, (0, 0, p, p, p, p)) if p else x
 
 
-def conv_ref(x, w, k, s):
-    """z = conv2d(x, w), padding (k - 1) // 2, as one DGEMM per tap"""
+def _chunks(n, chunk):
+    """batch slices of `chunk` images (all of them at once when chunk is None): the fp64 temporaries of a reference scale with the chunk"""
+    step = chunk or n
+    return [slice(i, min(n, i + step)) for i in range(0, n, step)]
+
+
+def conv_ref(x, w, k, s, chunk=None):
+    """z = conv2d(x, w), padding (k - 1) // 2, as one DGEMM per tap (per batch chunk)"""
     n, h, wd, cin = x.shape
     cout, p = w.shape[0], (k - 1) // 2
     oh, ow = h // s, wd // s
-    xp, xa = _pad(x, p), _pad(x.abs(), p)
-    ref = x.new_zeros(n * oh * ow, cout)
-    mag = x.new_zeros(n * oh * ow, cout)
-    for kh, kw, sl in _tap_slices(xp, k, s, oh, ow):
-        wt = w[:, :, kh, kw]
-        ref += xp[sl].reshape(-1, cin) @ wt.t()
-        mag += xa[sl].reshape(-1, cin) @ wt.abs().t()
-    return ref.view(n, oh, ow, cout), mag.view(n, oh, ow, cout), k * k * cin
+    ref = x.new_zeros(n, oh, ow, cout)
+    mag = x.new_zeros(n, oh, ow, cout)
+    for b in _chunks(n, chunk):
+        xp, xa = _pad(x[b], p), _pad(x[b].abs(), p)
+        r, m = ref[b].view(-1, cout), mag[b].view(-1, cout)
+        for kh, kw, sl in _tap_slices(xp, k, s, oh, ow):
+            wt = w[:, :, kh, kw]
+            r += xp[sl].reshape(-1, cin) @ wt.t()
+            m += xa[sl].reshape(-1, cin) @ wt.abs().t()
+    return ref, mag, k * k * cin
 
 
-def dgrad_ref(dz, w, k, s, xshape):
-    """dx = conv2d_input(dz, w): every tap's product scattered back to the input pixels it came from"""
+def dgrad_ref(dz, w, k, s, xshape, chunk=None):
+    """dx = conv2d_input(dz, w): every tap's product scattered back to the input pixels it came from (per batch chunk)"""
     n, h, wd, cin = xshape
     _, oh, ow, cout = dz.shape
     p = (k - 1) // 2
-    ref = dz.new_zeros(n, h + 2 * p, wd + 2 * p, cin)
-    mag = torch.zeros_like(ref)
-    d2, a2 = dz.reshape(-1, cout), dz.abs().reshape(-1, cout)
-    for kh, kw, sl in _tap_slices(ref, k, s, oh, ow):
-        wt = w[:, :, kh, kw]
-        ref[sl] += (d2 @ wt).view(n, oh, ow, cin)
-        mag[sl] += (a2 @ wt.abs()).view(n, oh, ow, cin)
+    out = dz.new_empty(n, h, wd, cin)
+    out_mag = torch.empty_like(out)
     crop = (slice(None), slice(p, p + h), slice(p, p + wd))
-    return ref[crop], mag[crop], k * k * cout
+    for b in _chunks(n, chunk):
+        nb = b.stop - b.start
+        ref = dz.new_zeros(nb, h + 2 * p, wd + 2 * p, cin)
+        mag = torch.zeros_like(ref)
+        d2, a2 = dz[b].reshape(-1, cout), dz[b].abs().reshape(-1, cout)
+        for kh, kw, sl in _tap_slices(ref, k, s, oh, ow):
+            wt = w[:, :, kh, kw]
+            ref[sl] += (d2 @ wt).view(nb, oh, ow, cin)
+            mag[sl] += (a2 @ wt.abs()).view(nb, oh, ow, cin)
+        out[b], out_mag[b] = ref[crop], mag[crop]
+    return out, out_mag, k * k * cout
 
 
-def wgrad_ref(x, dz, k, s):
-    """grad[co, ci, kh, kw] = sum over output pixels of dz * x(tap)"""
+def wgrad_ref(x, dz, k, s, chunk=None):
+    """grad[co, ci, kh, kw] = sum over output pixels of dz * x(tap); per batch chunk, the chunks' sums added"""
     cin, (n, oh, ow, cout) = x.shape[-1], dz.shape
     p = (k - 1) // 2
-    xp, xa = _pad(x, p), _pad(x.abs(), p)
-    d2, a2 = dz.reshape(-1, cout), dz.abs().reshape(-1, cout)
     ref = x.new_zeros(cout, cin, k, k)
     mag = torch.zeros_like(ref)
-    for kh, kw, sl in _tap_slices(xp, k, s, oh, ow):
-        ref[:, :, kh, kw] = d2.t() @ xp[sl].reshape(-1, cin)
-        mag[:, :, kh, kw] = a2.t() @ xa[sl].reshape(-1, cin)
+    for b in _chunks(n, chunk):
+        xp, xa = _pad(x[b], p), _pad(x[b].abs(), p)
+        d2, a2 = dz[b].reshape(-1, cout), dz[b].abs().reshape(-1, cout)
+        for kh, kw, sl in _tap_slices(xp, k, s, oh, ow):
+            ref[:, :, kh, kw] += d2.t() @ xp[sl].reshape(-1, cin)
+            mag[:, :, kh, kw] += a2.t() @ xa[sl].reshape(-1, cin)
     return ref, mag, n * oh * ow
 
 
@@ -247,7 +269,7 @@ def _fold_mask(cout, cin, group):
     return m
 
 
-def run_fwd(gx, gz, k, s, stats=True, fold=0, seed=1):
+def run_fwd(gx, gz, k, s, stats=True, fold=0, seed=1, chunk=None):
     """yb200_conv2d_fwd (fold > 0: yb200_conv2d_fwd_fold with stat_fold = fold): fp16 z and its BatchNorm statistics"""
     capi, L = _lib()
     g = _g(seed)
@@ -265,7 +287,7 @@ def run_fwd(gx, gz, k, s, stats=True, fold=0, seed=1):
     else:
         rc = L.yb200_conv2d_fwd(ctypes.byref(xa), capi.ptr(wf), ctypes.byref(za), k, s, ps, pq, capi.stream_ptr())
     capi.check(rc, "conv2d_fwd")
-    ref, mag, kk = conv_ref(_sl(x, gx).double(), w, k, s)
+    ref, mag, kk = conv_ref(_sl(x, gx).double(), w, k, s, chunk)
     zs = _sl(z, gz)
     check("fwd z (fp16)", zs, ref, bound(ref, mag, kk, R_F16), "z")
     _outside_same(z, z0, gz, "z")
@@ -278,7 +300,7 @@ def run_fwd(gx, gz, k, s, stats=True, fold=0, seed=1):
         _guard_ok(qb, nst, "sum of z^2")
 
 
-def run_bn_silu(gx, go, gr, k, s, seed=2):
+def run_bn_silu(gx, go, gr, k, s, seed=2, chunk=None):
     """yb200_conv2d_bn_silu_fwd: bf16(SiLU(conv * scale + shift)) [+ residual, after rounding the activation]"""
     capi, L = _lib()
     g = _g(seed)
@@ -293,7 +315,7 @@ def run_bn_silu(gx, go, gr, k, s, seed=2):
     ra = _act(capi, res, gr) if gr else None
     capi.check(L.yb200_conv2d_bn_silu_fwd(ctypes.byref(xa), capi.ptr(wf), capi.ptr(scale), capi.ptr(shift), ctypes.byref(ra) if gr else None,
                                           ctypes.byref(oa), k, s, capi.stream_ptr()), "conv2d_bn_silu_fwd")
-    zc, mag, kk = conv_ref(_sl(x, gx).double(), w, k, s)
+    zc, mag, kk = conv_ref(_sl(x, gx).double(), w, k, s, chunk)
     u = zc * scale.double() + shift.double()
     act = u * torch.sigmoid(u)
     mag = 1.1 * (mag * scale.double() + shift.double().abs())  # |SiLU'| <= 1.1
@@ -305,7 +327,7 @@ def run_bn_silu(gx, go, gr, k, s, seed=2):
     _outside_same(out, out0, go, "out")
 
 
-def run_affine(gx, go, gr, k, s, with_scale=True, with_shift=True, seed=3):
+def run_affine(gx, go, gr, k, s, with_scale=True, with_shift=True, seed=3, chunk=None):
     """yb200_conv2d_affine_fwd: bf16(conv * scale + shift [+ residual])"""
     capi, L = _lib()
     g = _g(seed)
@@ -320,7 +342,7 @@ def run_affine(gx, go, gr, k, s, with_scale=True, with_shift=True, seed=3):
     ra = _act(capi, res, gr) if gr else None
     capi.check(L.yb200_conv2d_affine_fwd(ctypes.byref(xa), capi.ptr(wf), capi.ptr(scale), capi.ptr(shift), ctypes.byref(ra) if gr else None,
                                          ctypes.byref(oa), k, s, capi.stream_ptr()), "conv2d_affine_fwd")
-    ref, mag, kk = conv_ref(_sl(x, gx).double(), w, k, s)
+    ref, mag, kk = conv_ref(_sl(x, gx).double(), w, k, s, chunk)
     if scale is not None:
         ref, mag = ref * scale.double(), mag * scale.double()
     if shift is not None:
@@ -332,7 +354,7 @@ def run_affine(gx, go, gr, k, s, with_scale=True, with_shift=True, seed=3):
     _outside_same(out, out0, go, "out")
 
 
-def run_dgrad(gdz, gdx, ga, k, s, seed=4):
+def run_dgrad(gdz, gdx, ga, k, s, seed=4, chunk=None):
     """yb200_conv2d_dgrad: bf16(conv2d_input(dz, w) [+ addend])"""
     capi, L = _lib()
     g = _g(seed)
@@ -345,7 +367,7 @@ def run_dgrad(gdz, gdx, ga, k, s, seed=4):
     aa = _act(capi, add, ga) if ga else None
     capi.check(L.yb200_conv2d_dgrad(ctypes.byref(dza), capi.ptr(wd), ctypes.byref(dxa), ctypes.byref(aa) if ga else None, k, s,
                                     capi.stream_ptr()), "conv2d_dgrad")
-    ref, mag, kk = dgrad_ref(_sl(dz, gdz).double(), w, k, s, (gdx[0], gdx[1], gdx[2], cin))
+    ref, mag, kk = dgrad_ref(_sl(dz, gdz).double(), w, k, s, (gdx[0], gdx[1], gdx[2], cin), chunk)
     if ga:
         av = _sl(add, ga).double()
         ref, mag = ref + av, mag + av.abs()
@@ -353,7 +375,7 @@ def run_dgrad(gdz, gdx, ga, k, s, seed=4):
     _outside_same(dx, dx0, gdx, "dx")
 
 
-def run_wgrad(gx, gdz, k, s, cin_real=None, accumulate=0, group=0, repeat=False, seed=5):
+def run_wgrad(gx, gdz, k, s, cin_real=None, accumulate=0, group=0, repeat=False, seed=5, chunk=None):
     """yb200_conv2d_wgrad (group > 1: _wgrad_grouped): fp32 [cout][cin_real][k][k], split-K partials reduced in a fixed order"""
     capi, L = _lib()
     g = _g(seed)
@@ -378,7 +400,7 @@ def run_wgrad(gx, gdz, k, s, cin_real=None, accumulate=0, group=0, repeat=False,
         capi.check(rc, "conv2d_wgrad")
 
     call(grad, accumulate)
-    ref, mag, kk = wgrad_ref(_sl(x, gx).double(), _sl(dz, gdz).double(), k, s)
+    ref, mag, kk = wgrad_ref(_sl(x, gx).double(), _sl(dz, gdz).double(), k, s, chunk)
     ref, mag = ref[:, :cin_real], mag[:, :cin_real]
     got = grad
     if accumulate:
@@ -450,7 +472,7 @@ def run_dgrad_gelu(gdz, gu, gdu, bias_sum=True, seed=7):
         _guard_ok(sb, hid, "bias-gradient sums")
 
 
-def run_pred(gx, cout, a_total, a_off, c_total, c_off, seed=8):
+def run_pred(gx, cout, a_total, a_off, c_total, c_off, seed=8, chunk=None):
     """yb200_conv1x1_bias_f32: fp32 rows [n][a_total][c_total], block [a_off + pixel][c_off + c]"""
     capi, L = _lib()
     g = _g(seed)
@@ -465,7 +487,7 @@ def run_pred(gx, cout, a_total, a_off, c_total, c_off, seed=8):
     xa = _act(capi, x, gx)
     capi.check(L.yb200_conv1x1_bias_f32(ctypes.byref(xa), capi.ptr(wf), capi.ptr(b), cout, capi.ptr(out), a_total, a_off, c_total, c_off,
                                         capi.stream_ptr()), "conv1x1_bias_f32")
-    ref, mag, kk = conv_ref(_sl(x, gx).double(), w, 1, 1)
+    ref, mag, kk = conv_ref(_sl(x, gx).double(), w, 1, 1, chunk)
     ref, mag = (ref + b.double()).reshape(n, h * w_, cout), (mag + b.double().abs()).reshape(n, h * w_, cout)
     check("prediction conv (fp32)", out[blk], ref, bound(ref, mag, kk, 0.0), "out")
     out[blk] = 0

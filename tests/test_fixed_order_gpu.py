@@ -57,6 +57,11 @@ SPP_SHAPES = [
 @pytest.mark.parametrize("ties", [False, True], ids=["random", "many_ties"])
 @pytest.mark.parametrize("shape", SPP_SHAPES, ids=lambda s: "x".join(map(str, s)))
 def test_spp_pool_bwd_against_fp64(cuda, shape, ties):
+    check_spp_pool(cuda, shape, ties)
+
+
+def check_spp_pool(cuda, shape, ties):
+    """yb200_spp_pool (maxima and argmax bytes) and yb200_spp_pool_bwd on an [n, c, h, w] map, against fp64 max pooling and its autograd"""
     from yolov7_d2_b200 import capi
 
     L = capi.lib()

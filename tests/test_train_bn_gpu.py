@@ -566,13 +566,11 @@ def test_pack_weights_batched_synthetic_table(cuda):
 
 # ------------------------------------------------------------------------------------------------ every BatchNorm of a real step
 
-@pytest.fixture(scope="module")
-def step(cuda):
-    """YOLOX-s at 8 x 256 after one train_step(), non-trivial BatchNorm affine parameters and running statistics.  Snapshots of what a
-    second step changes (running statistics, gradients) are kept, so the tests below do not depend on each other's order."""
+def build_step(cuda, batch, size):
+    """YOLOX-s at batch x size^2 after one train_step(), non-trivial BatchNorm affine parameters and running statistics.  Snapshots of
+    what a second step changes (running statistics, gradients) are kept, so the checks do not depend on each other's order."""
     from yolov7_d2_b200.engine import YoloxEngine
 
-    batch, size = 8, 256
     sd = orc.yolox_state_dict(3)
     g = torch.Generator().manual_seed(9)
     for k in sd:
@@ -591,7 +589,13 @@ def step(cuda):
     eng.labels.copy_(labels.to(cuda))
     eng.train_step()
     torch.cuda.synchronize()
-    return dict(eng=eng, sd=sd, rm=eng.flat_rm.clone(), rv=eng.flat_rv.clone(), grad=eng.flat_grad.clone(), stats=eng.flat_stats.clone())
+    return dict(eng=eng, sd=sd, rm=eng.flat_rm.clone(), rv=eng.flat_rv.clone(), grad=eng.flat_grad.clone(), stats=eng.flat_stats.clone(),
+                images=images, labels=labels)
+
+
+@pytest.fixture(scope="module")
+def step(cuda):
+    return build_step(cuda, 8, 256)
 
 
 def _heads(eng):
@@ -621,21 +625,28 @@ def _layer_refs(eng, op, hd, stats):
     return z, P, (stats[o:o + c], stats[nb + o:nb + o + c]), consts, _bwd_ref(z, d, d_abs, d_adds, *consts, _red_path(c, P))
 
 
-def test_step_every_batchnorm_against_fp64(step):
-    """For every BatchNorm of the step: the convolution epilogue's sums of the stored z, the published constants, the running
-    statistics against the loaded ones, the activation (+ residual, + upsampled copy), dz, and the weight / bias gradients at the
-    per-head parameter (gamma offset by hd.c0, bn_goff / bn_boff)"""
+def _all_tiles(eng, op):
+    """every 128-pixel tile of the layer's output grid (the stem's tiles cover its [n, h, w / 4] grouped grid): a bound on the tiles
+    one CTA walks"""
+    zb = op.z.buf
+    return _choose_tile(zb.n, zb.h, zb.w // 4) if (op.first and eng.group4) else _choose_tile(zb.n, zb.h, zb.w)
+
+
+def check_every_batchnorm(step, tiles_per_cta=_all_tiles, layers=None):
+    """For every BatchNorm of the step (or those named in `layers`): the convolution epilogue's sums of the stored z, the published
+    constants, the running statistics against the loaded ones, the activation (+ residual, + upsampled copy), dz, and the weight / bias
+    gradients at the per-head parameter (gamma offset by hd.c0, bn_goff / bn_boff).  tiles_per_cta(eng, op): the most tiles one CTA
+    of the layer's forward walks."""
     eng, sd = step["eng"], step["sd"]
-    nb = eng.nbn
     for op, hd in _heads(eng):
         name = hd.prefix
+        if layers is not None and name not in layers:
+            continue
         z, P, (S, Q), (scale, shift, mean_k, invstd_k), r = _layer_refs(eng, op, hd, step["stats"])
         c = hd.c
         # sums: fp32 per warp (32 pixels, 5 butterfly levels), one addition per 128-pixel tile the CTA walks, two levels for the four
-        # 32-pixel quadrants, fp64 atomics (negligible); squares round once more.  The stem's tiles cover its [n, h, w / 4] grouped grid.
-        zb = op.z.buf
-        tiles = _choose_tile(zb.n, zb.h, zb.w // 4) if (op.first and eng.group4) else _choose_tile(zb.n, zb.h, zb.w)
-        k = 5 + tiles + 2
+        # 32-pixel quadrants, fp64 atomics (negligible); squares round once more
+        k = 5 + tiles_per_cta(eng, op) + 2
         _fail(name, "stat_sum", (S - z.sum(0)).abs(), k * U32 * z.abs().sum(0))
         _fail(name, "stat_sqsum", (Q - (z * z).sum(0)).abs(), (k + 1) * U32 * (z * z).sum(0))
         gamma, beta = eng.params[name + ".bn.weight"], eng.params[name + ".bn.bias"]
@@ -653,6 +664,13 @@ def test_step_every_batchnorm_against_fp64(step):
         bofs = (eng.grads[name + ".bn.bias"].data_ptr() - eng.flat_grad.data_ptr()) // 4
         _check_param(name, "bn.weight grad", step["grad"][gofs:gofs + c], r["dg"], r["e_dg"])
         _check_param(name, "bn.bias grad", step["grad"][bofs:bofs + c], r["db"], r["e_db"])
+        del z, r
+
+
+def test_step_every_batchnorm_against_fp64(step):
+    eng = step["eng"]
+    nb = eng.nbn
+    check_every_batchnorm(step)
     assert (step["stats"][2 * nb:] == 0).all(), "the dgamma / dbeta accumulators are not zero after backward"
     _check_head_bias(eng, step["grad"], None)
     hc = eng.hc

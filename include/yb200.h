@@ -512,6 +512,40 @@ int yb200_resize_bilinear_bwd(const yb200_act* dout, const yb200_act* h, const y
 int yb200_upsample_nearest2x_add(const yb200_act* lat, const yb200_act* coarse, const yb200_act* out, void* stream);
 int yb200_upsample_nearest2x_bwd(const yb200_act* dy, const yb200_act* h, const yb200_act* dx, void* stream);
 
+/* ---- SparseInst meta-architecture: input and inference (yolov7/modeling/meta_arch/sparseinst.py) --------------------------------------------
+ * Fixed summation order and no float atomics in every call below: bit-reproducible.
+ *   yb200_normalize_pad: preprocess_inputs (:96-100) for a batch: images [3][h][w] uint8 (is_f32 = 0) or fp32 (is_f32 = 1) staged in one device
+ *     buffer; table: DEVICE int64 [n][3] = (element offset, h, w) per image, every h <= hp, w <= wp.  out fp32 [n][3][hp][wp] =
+ *     (float(x) - mean[c]) / std[c] (one IEEE subtract and one IEEE divide: the bits of torch's arithmetic), 0 beyond each image (the pad value
+ *     of ImageList.from_tensors).  mean, std: DEVICE fp32 [3].
+ *   yb200_sparseinst_infer_scores: the scores of `inference` (:179-213) for a batch.  logits fp32 [B][N][K], scores fp32 [B][N] (the
+ *     objectness logits), masks fp32 [B][N][HW] (the mask logits).  Per (image, query), in fp32: v_k = sqrt(sigmoid(l_k) * sigmoid(s)),
+ *     score = max_k v_k and label = the lowest k attaining it, keep = score > cls_threshold, and for kept queries, with m = sigmoid(mask),
+ *     rescored = score * (Σ m [m > mask_threshold] / (Σ [m > mask_threshold] + 1e-6)) (rescoring_mask, :24-27; 0 for the others).  Writes
+ *     score, label int32, keep uint8 and rescored, all [B][N]; then counts int32 [B] of kept queries, exclusive offsets int32 [B + 1]
+ *     (offsets[B] = their total), and in compact order (image, then ascending query) kept_query int32 (the query's index within its image),
+ *     kept_score fp32 (rescored) and kept_label int64, each with room for B * N entries.
+ *   yb200_sparseinst_paste_masks: the masks of `inference` (:215-232) for every kept query of up to YB200_PASTE_MAX_IMAGES images in one
+ *     launch.  masks fp32 [B][N][Hm][Wm] (the logits), kept_query as written above, images: HOST array of B descriptors; image b's kept masks
+ *     are compact entries [first, first + count), with first = the sum of the counts before it.  For each output pixel of the (out_h, out_w)
+ *     original size: sigmoid, F.interpolate(bilinear, align_corners=False) to (hp, wp), crop to (h, w), F.interpolate to (out_h, out_w), then
+ *     > mask_threshold, written as uint8 [count][out_h][out_w] at byte offset out_off of `out`.  Both resizes use ATen's index arithmetic
+ *     (scale = in / out, src = max(scale (dst + 0.5) - 0.5, 0), i1 = i0 + (i0 < in - 1), fp32 weights); the intermediates stay in shared memory. */
+#define YB200_PASTE_MAX_IMAGES 64
+typedef struct yb200_paste_image {
+  int32_t h, w;          /* the image's size inside the padded batch (the crop) */
+  int32_t out_h, out_w;  /* the original size ("height", "width") */
+  int32_t first, count;  /* its kept masks in compact order */
+  int64_t out_off;       /* byte offset of its [count][out_h][out_w] output */
+} yb200_paste_image;
+int yb200_normalize_pad(const void* images, int is_f32, const int64_t* table, int n, const float* mean, const float* std, int hp, int wp,
+                        float* out, void* stream);
+int yb200_sparseinst_infer_scores(const float* logits, const float* scores, const float* masks, int B, int N, int K, int HW, float cls_threshold,
+                                  float mask_threshold, float* score, int32_t* label, uint8_t* keep, float* rescored, int32_t* counts,
+                                  int32_t* offsets, int32_t* kept_query, float* kept_score, int64_t* kept_label, void* stream);
+int yb200_sparseinst_paste_masks(const float* masks, int N, int Hm, int Wm, const int32_t* kept_query, const yb200_paste_image* images, int B,
+                                 int hp, int wp, float mask_threshold, uint8_t* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -546,6 +546,37 @@ int yb200_sparseinst_infer_scores(const float* logits, const float* scores, cons
 int yb200_sparseinst_paste_masks(const float* masks, int N, int Hm, int Wm, const int32_t* kept_query, const yb200_paste_image* images, int B,
                                  int hp, int wp, float mask_threshold, uint8_t* out, void* stream);
 
+/* ---- DETR meta-architecture: masks, positions, targets and inference (yolov7/modeling/meta_arch/detr.py) ------------------------------------
+ * No float atomics and fixed-order sums in every call below: bit-reproducible.  The input normalisation is yb200_normalize_pad.
+ *   yb200_detr_mask_pos: MaskedBackboneTraceFriendly.mask_out_padding (:389-403) and PositionEmbeddingSine(normalize=True) (detr_backbone.py
+ *     :334-375) for every level of the backbone in one launch.  levels: HOST array of nlevels (<= YB200_DETR_MAX_LEVELS) descriptors; valid:
+ *     DEVICE int32 [nlevels][B][2] = (rows, cols) of image b's valid top-left rectangle at that level (ceil(h / stride), ceil(w / stride),
+ *     clamped to the level's size); dim_t: DEVICE fp32 [npf] = temperature ** (2 (i // 2) / npf), npf even.  Writes mask bool [B][h][w] (1
+ *     outside the rectangle) and pos fp32 [B][2 npf][h][w]: the y half, then the x half, sin on even channels and cos on odd ones of
+ *     (e / (last + 1e-6) * fp32(2 pi)) / dim_t, with e the cumulative count of valid pixels along the axis and last its final value.
+ *   yb200_detr_infer: `inference` (:219-265) and detectron2's detector_postprocess for a batch.  logits fp32 [B][Q][K1], boxes fp32 [B][Q][4]
+ *     (cx, cy, w, h), sizes DEVICE fp32 [B][6] = (image w, image h, fp32(out w / image w), fp32(out h / image h), out w, out h).  Per row:
+ *     score = max over k < K1 - 1 of softmax(logits) (label = the lowest k attaining it); xyxy = (cx - 0.5 w, cy - 0.5 h, cx + 0.5 w,
+ *     cy + 0.5 h), times the image size, times the ratios, clamped to [0, out w] x [0, out h]; kept when score > threshold and the clamped box
+ *     has positive width and height.  Writes score, label int32, keep uint8 (bit 0: kept; bit 1: score > threshold and a coordinate not
+ *     finite), box fp32 [4] (the clamped xyxy), all per row; counts int32 [B], exclusive offsets int32 [B + 1], status int32 [1] (the OR of
+ *     keep >> 1 over the batch), and in compact order (image, then ascending query) kept_query int32, kept_score fp32, kept_label int64 and
+ *     kept_box fp32 [4], each with room for B * Q entries.
+ *   yb200_detr_pack_targets: `prepare_targets` (:204-217) for a batch.  boxes fp32 [G][4] (gt_boxes XYXY, absolute), table DEVICE int32
+ *     [B][4] = (first box, box count, h, w) per image.  out fp32 [G][4] = box_xyxy_to_cxcywh(box / [w, h, w, h]): ((x0 + x1) / 2,
+ *     (y0 + y1) / 2, x1 - x0, y1 - y0) after the four IEEE divides. */
+#define YB200_DETR_MAX_LEVELS 8
+typedef struct yb200_detr_level {
+  uint8_t* mask; /* bool [B][h][w] */
+  float* pos;    /* fp32 [B][2 npf][h][w] */
+  int32_t h, w;  /* the level's feature size */
+} yb200_detr_level;
+int yb200_detr_mask_pos(const yb200_detr_level* levels, int nlevels, int B, const int32_t* valid, const float* dim_t, int npf, void* stream);
+int yb200_detr_infer(const float* logits, const float* boxes, int B, int Q, int K1, const float* sizes, float threshold, float* score, int32_t* label,
+                     uint8_t* keep, float* box, int32_t* counts, int32_t* offsets, int32_t* kept_query, float* kept_score, int64_t* kept_label,
+                     float* kept_box, int32_t* status, void* stream);
+int yb200_detr_pack_targets(const float* boxes, const int32_t* table, int B, int G, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -3,6 +3,7 @@
 // two bilinear resizes of every kept mask (to the padded input, crop, to the original size) fused with the mask threshold.  Every sum runs in
 // a fixed order and there are no float atomics: the results are bit-reproducible.
 #include "host_common.cuh"
+#include "infer_compact.cuh"
 #include "sm90.cuh"
 
 #include <math.h>
@@ -88,38 +89,6 @@ __global__ void __launch_bounds__(kScoreThreads) infer_scores_kernel(const float
     __syncthreads();
   }
   if (threadIdx.x == 0) rescored[row] = s_score * (s_sum[0] / (s_cnt[0] + 1e-6f));
-}
-
-// The kept queries of the batch in compact order (image, then ascending query): counts [B], exclusive offsets [B + 1], and per kept query its
-// index within the image, its rescored score and its label as int64.  One CTA; thread b owns image b.
-__global__ void __launch_bounds__(256) infer_compact_kernel(const uint8_t* __restrict__ keep, const float* __restrict__ rescored,
-                                                            const int32_t* __restrict__ label, int B, int N, int32_t* __restrict__ counts,
-                                                            int32_t* __restrict__ offsets, int32_t* __restrict__ kept_query,
-                                                            float* __restrict__ kept_score, int64_t* __restrict__ kept_label) {
-  pdl_sync();
-  for (int b = threadIdx.x; b < B; b += blockDim.x) {
-    int c = 0;
-    for (int q = 0; q < N; ++q) c += keep[static_cast<long long>(b) * N + q];
-    counts[b] = c;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int run = 0;
-    for (int b = 0; b < B; ++b) offsets[b] = run, run += counts[b];
-    offsets[B] = run;
-  }
-  __syncthreads();
-  for (int b = threadIdx.x; b < B; b += blockDim.x) {
-    int j = offsets[b];
-    for (int q = 0; q < N; ++q) {
-      const long long r = static_cast<long long>(b) * N + q;
-      if (!keep[r]) continue;
-      kept_query[j] = q;
-      kept_score[j] = rescored[r];
-      kept_label[j] = label[r];
-      ++j;
-    }
-  }
 }
 
 // ATen's upsample_bilinear2d source index (align_corners=False, size given): scale = in / out, src = max(scale (dst + 0.5) - 0.5, 0),
@@ -239,7 +208,8 @@ extern "C" int yb200_sparseinst_infer_scores(const float* logits, const float* s
   launch_k(infer_scores_kernel, B * N, kScoreThreads, 0, st, logits, scores, masks, K, HW, cls_threshold, mask_threshold, score, label, keep, rescored);
   YB_CHECK_CUDA(cudaGetLastError());
   launch_k(infer_compact_kernel, 1, 256, 0, st, static_cast<const uint8_t*>(keep), static_cast<const float*>(rescored),
-           static_cast<const int32_t*>(label), B, N, counts, offsets, kept_query, kept_score, kept_label);
+           static_cast<const int32_t*>(label), static_cast<const float*>(nullptr), B, N, counts, offsets, kept_query, kept_score, kept_label,
+           static_cast<float*>(nullptr), static_cast<int32_t*>(nullptr));
   YB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -20,6 +20,7 @@ import torch
 import torch.nn as nn
 
 from . import capi
+from .batch_input import normalize_pad
 from .modeling import BACKBONE_REGISTRY, HAVE_D2, META_ARCH_REGISTRY, Instances, ShapeSpec
 from .sparseinst import BaseIAMDecoder, GroupIAMDecoder
 from .sparseinst_criterion import build_sparse_inst_criterion
@@ -57,10 +58,6 @@ class PasteImage(ctypes.Structure):
 PASTE_MAX_IMAGES = 64  # YB200_PASTE_MAX_IMAGES
 
 
-def _pinned_to(arr, device):
-    return torch.from_numpy(np.ascontiguousarray(arr)).pin_memory().to(device, non_blocking=True)
-
-
 @META_ARCH_REGISTRY.register()
 class SparseInst(nn.Module):
     def __init__(self, cfg):
@@ -93,28 +90,7 @@ class SparseInst(nn.Module):
     # ---- input -------------------------------------------------------------------------------------------------------------------
     def preprocess_inputs(self, batched_inputs):
         """fp32 [B, 3, Hp, Wp] normalised and zero-padded to a multiple of 32, and the images' (h, w)"""
-        imgs = [x["image"] for x in batched_inputs]
-        if not imgs:
-            raise capi.Yb200Error("SparseInst: empty batch")
-        for i, im in enumerate(imgs):
-            if im.dim() != 3 or im.shape[0] != 3 or im.dtype not in (torch.uint8, torch.float32) or im.numel() == 0:
-                raise capi.Yb200Error(f"SparseInst: image {i} is {tuple(im.shape)} {im.dtype} (expected [3, H, W] uint8 or float32)")
-        is_f32 = any(im.dtype == torch.float32 for im in imgs)
-        dtype = torch.float32 if is_f32 else torch.uint8
-        sizes = [(int(im.shape[1]), int(im.shape[2])) for im in imgs]
-        s = SIZE_DIVISIBILITY
-        hp = (max(h for h, _ in sizes) + s - 1) // s * s
-        wp = (max(w for _, w in sizes) + s - 1) // s * s
-        counts = [im.numel() for im in imgs]
-        offs = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
-        staged = torch.empty(int(offs[-1]), dtype=dtype, device=self.device)
-        for im, o, n in zip(imgs, offs, counts):
-            staged[int(o):int(o) + n].copy_(im.reshape(-1), non_blocking=True)  # one copy per image; uint8 -> fp32 is exact
-        table = _pinned_to(np.array([(o, h, w) for o, (h, w) in zip(offs[:-1], sizes)], dtype=np.int64), self.device)
-        out = torch.empty(len(imgs), 3, hp, wp, device=self.device)
-        capi.check(self.L.yb200_normalize_pad(capi.ptr(staged), int(is_f32), capi.ptr(table), len(imgs), capi.ptr(self.pixel_mean),
-                                              capi.ptr(self.pixel_std), hp, wp, capi.ptr(out), capi.stream_ptr()), "normalize_pad")
-        return out, sizes
+        return normalize_pad(self.L, [x["image"] for x in batched_inputs], self.pixel_mean, self.pixel_std, SIZE_DIVISIBILITY, "SparseInst")
 
     def prepare_targets(self, targets):
         """:102-120: per image {"labels": int64 on the device, "masks": BitMasks on the device}"""

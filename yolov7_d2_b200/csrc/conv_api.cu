@@ -11,10 +11,42 @@ namespace yb {
 // ------------------------------------------------------------------------------------------------
 // kernel dispatch
 // ------------------------------------------------------------------------------------------------
+// Tensor maps of the TMA-store epilogue (ConvOutMaps) from the output geometry of `p`: the (n, y, x) -> offset mapping of the output and of
+// the addend, over the work items' pixel grid with its valid extents, and the output's own channels; the box is the 64-row half tile of one
+// consumer warpgroup.  A four-phase data gradient gets one map per output-parity phase, the phase's offset in its base.
+static int make_out_maps(ConvOutMaps* om, const ConvGemmParams& p, int bn) {
+  YB_REQUIRE(p.out_sc == 1, YB200_ERR_INVALID, "conv: a 16-bit output needs channel stride 1");
+  int hx, hy, hn;
+  conv_half_offset(p.log_tw, p.log_th, hx, hy, hn);
+  const int tw = 1 << p.log_tw, th = 1 << p.log_th, tn = 128 >> (p.log_tw + p.log_th);
+  const int bw = hx ? tw / 2 : tw, bh = hy ? th / 2 : th, bnn = hn ? tn / 2 : tn;
+  const int box_c = bn < 64 ? bn : 64;
+  for (int ph = 0; ph < (p.num_phases == 4 ? 4 : 1); ++ph) {
+    const int oph = ph >> 1, opw = ph & 1;
+    const char* out = static_cast<const char*>(p.out) + 2 * (oph * p.out_sh + opw * p.out_sw);
+    int rc = make_pix_map(&om->out[ph], out, p.cout, p.w_valid, p.h_valid, p.n_valid, p.out_mw * p.out_sw, p.out_mh * p.out_sh, p.out_sn, box_c,
+                          bw, bh, bnn);
+    if (rc) return rc;
+    if (p.addend == nullptr) continue;
+    const char* add = reinterpret_cast<const char*>(p.addend) + 2 * (oph * p.add_sh + opw * p.add_sw);
+    rc = make_pix_map(&om->add[ph], add, p.cout, p.w_valid, p.h_valid, p.n_valid, p.out_mw * p.add_sw, p.out_mh * p.add_sh, p.add_sn, box_c, bw,
+                      bh, bnn);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
 template <int BN, int BK>
 static int launch_conv_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvGemmParams& p, dim3 grid, cudaStream_t st) {
   using Cfg = ConvGemmCfg<BN, BK>;
   const bool ext = p.epi_mode >= EPI_BF16_AFFINE;  // ConvNeXt / transformer epilogues live in their own instantiations
+  // the 16-bit YOLOX modes store through tensor maps (the TMA-store epilogue of conv_gemm_persistent_kernel)
+  ConvOutMaps om;
+  memset(&om, 0, sizeof(om));
+  if (!ext && p.epi_mode != EPI_F32_BIAS) {
+    const int rc = make_out_maps(&om, p, BN);
+    if (rc) return rc;
+  }
   // persistent kernel: one or two CTAs per SM as its launch bounds (conv_min_ctas); the ring is as deep as the CTA's share of shared
   // memory allows after the epilogue staging tiles
   const int phases = p.num_phases == 4 ? 4 : 1;
@@ -45,9 +77,9 @@ static int launch_conv_inst(const CUtensorMap& tmA, const CUtensorMap& tmB, cons
   ConvGemmParams pp = p;
   pp.xpose = xpose ? 1 : 0;
   if (ext)
-    launch_k(conv_gemm_persistent_kernel<BN, BK, true>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, pp, pst, kbs, n_tiles, m_tiles);
+    launch_k(conv_gemm_persistent_kernel<BN, BK, true>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, pp, om, pst, kbs, n_tiles, m_tiles);
   else
-    launch_k(conv_gemm_persistent_kernel<BN, BK, false>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, pp, pst, kbs, n_tiles, m_tiles);
+    launch_k(conv_gemm_persistent_kernel<BN, BK, false>, groups * n_tiles, kConvThreadsP, smem, st, tmA, tmB, pp, om, pst, kbs, n_tiles, m_tiles);
   YB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -129,14 +129,6 @@ __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
   __half2 v = __floats2half2_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
 }
-__device__ __forceinline__ void store_f16x8(__half* dst, const float* v) {
-  uint4 u;
-  u.x = pack_f16x2(v[0], v[1]);
-  u.y = pack_f16x2(v[2], v[3]);
-  u.z = pack_f16x2(v[4], v[5]);
-  u.w = pack_f16x2(v[6], v[7]);
-  *reinterpret_cast<uint4*>(dst) = u;
-}
 __device__ __forceinline__ void store_bf16x8(__nv_bfloat16* dst, const float* v) {
   uint4 u;
   u.x = pack_bf16x2(v[0], v[1]);
@@ -146,9 +138,6 @@ __device__ __forceinline__ void store_bf16x8(__nv_bfloat16* dst, const float* v)
   *reinterpret_cast<uint4*>(dst) = u;
 }
 
-// One chunk (CH columns of one accumulator row per lane) of the epilogue.
-//   part_sum / part_sq: this warp's shared-memory slots for the chunk's columns (EPI_F16_STATS); `accumulate` adds to them
-//   (statistics over all tiles of the CTA) instead of overwriting.
 // Per-column parameters (scale | shift / bias) of the CTA's column tile are staged in shared memory once per CTA; the epilogue reads
 // them with 16-byte broadcast loads (per-element __ldg plus a null test per element made the parameterised epilogues 2-3x slower
 // than the plain one).  Columns beyond cout hold (1, 0).
@@ -169,10 +158,14 @@ __device__ __forceinline__ void stage_col_params(const ConvGemmParams& p, int co
 constexpr int kXposeWarpFloats = 32 * 33 + 64;              // 32 x 32 chunk (pitch 33: conflict free both ways) + 32 row offsets (8 B each)
 constexpr int kXposeBytes = 8 * kXposeWarpFloats * 4;       // eight epilogue warps
 
+// One chunk (CH columns of one accumulator row per lane) of the staging-tile epilogue: EPI_F32_BIAS and, with EXT, the ConvNeXt /
+// transformer modes (the 16-bit YOLOX modes store from the accumulator fragments: conv_gemm_persistent_kernel).
+//   part_sum: this warp's shared-memory slots for the chunk's columns (column sums of EPI_BF16_GELU_BWD / EPI_BF16_RELU_BWD); `accumulate`
+//   adds to them (sums over all tiles of the CTA) instead of overwriting.
 template <int CH, bool EXT = true>
 __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, float (&v)[CH], bool valid, long long pix_off, long long add_off,
-                                                    int cbase, int lane, float* part_sum, float* part_sq, bool accumulate,
-                                                    const float* col_scale, const float* col_shift, float* xp = nullptr) {
+                                                    int cbase, int lane, float* part_sum, bool accumulate, const float* col_scale,
+                                                    const float* col_shift, float* xp = nullptr) {
   if (p.epi_mode == EPI_F32_BIAS) {
     if (xp != nullptr) {
       long long* s_off = reinterpret_cast<long long*>(xp + 32 * 33);
@@ -197,18 +190,6 @@ __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, flo
         if (cbase + i < p.cout) o[(long long)(cbase + i) * p.out_sc] = v[i] + col_shift[i];
     }
     return;
-  }
-  if (p.epi_mode == EPI_BF16_BN_SILU) {
-#pragma unroll
-    for (int i = 0; i < CH; i += 4) {
-      const float4 sc = *reinterpret_cast<const float4*>(col_scale + i), sh = *reinterpret_cast<const float4*>(col_shift + i);
-      const float u0 = fmaf(v[i], sc.x, sh.x), u1 = fmaf(v[i + 1], sc.y, sh.y), u2 = fmaf(v[i + 2], sc.z, sh.z), u3 = fmaf(v[i + 3], sc.w, sh.w);
-      // rounded before the residual add, as a materialised activation
-      v[i] = bf16_round(__fdividef(u0, 1.f + __expf(-u0)));
-      v[i + 1] = bf16_round(__fdividef(u1, 1.f + __expf(-u1)));
-      v[i + 2] = bf16_round(__fdividef(u2, 1.f + __expf(-u2)));
-      v[i + 3] = bf16_round(__fdividef(u3, 1.f + __expf(-u3)));
-    }
   }
   if constexpr (EXT) {
     if (p.epi_mode == EPI_BF16_AFFINE) {
@@ -278,45 +259,20 @@ __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, flo
         }
       }
     }
-  }
-  if (p.addend != nullptr && valid) {
-    const __nv_bfloat16* a = p.addend + add_off + cbase;
+      if (p.addend != nullptr && valid) {
+      const __nv_bfloat16* a = p.addend + add_off + cbase;
 #pragma unroll
-    for (int i = 0; i < CH; i += 8) {
-      if (cbase + i < p.cout) {
-        const uint4 u = *reinterpret_cast<const uint4*>(a + i);
-        v[i + 0] += bf16_lo(u.x); v[i + 1] += bf16_hi(u.x);
-        v[i + 2] += bf16_lo(u.y); v[i + 3] += bf16_hi(u.y);
-        v[i + 4] += bf16_lo(u.z); v[i + 5] += bf16_hi(u.z);
-        v[i + 6] += bf16_lo(u.w); v[i + 7] += bf16_hi(u.w);
+      for (int i = 0; i < CH; i += 8) {
+        if (cbase + i < p.cout) {
+          const uint4 u = *reinterpret_cast<const uint4*>(a + i);
+          v[i + 0] += bf16_lo(u.x); v[i + 1] += bf16_hi(u.x);
+          v[i + 2] += bf16_lo(u.y); v[i + 3] += bf16_hi(u.y);
+          v[i + 4] += bf16_lo(u.z); v[i + 5] += bf16_hi(u.z);
+          v[i + 6] += bf16_lo(u.w); v[i + 7] += bf16_hi(u.w);
+        }
       }
     }
-  }
-  // round once (one packed conversion per two values; the kernels that carry this epilogue are bound by its instruction count on the narrow
-  // layers, ncu: ~50 % issue-slot utilisation with 8 epilogue warps per CTA); statistics describe exactly the values that are stored
-  const bool f16 = p.epi_mode == EPI_F16 || p.epi_mode == EPI_F16_STATS;
-  const bool need_vals = p.epi_mode == EPI_F16_STATS || (EXT && p.stat_sum != nullptr);
-  if (f16) {
-    uint32_t pk[CH / 2];
-#pragma unroll
-    for (int i = 0; i < CH; i += 2) pk[i >> 1] = pack_f16x2(v[i], v[i + 1]);
-    if (valid) {
-      __half* o = reinterpret_cast<__half*>(p.out) + pix_off + cbase;
-#pragma unroll
-      for (int i = 0; i < CH; i += 8)
-        if (cbase + i < p.cout) *reinterpret_cast<uint4*>(o + i) = make_uint4(pk[i >> 1], pk[(i >> 1) + 1], pk[(i >> 1) + 2], pk[(i >> 1) + 3]);
-    }
-    if (need_vals) {
-#pragma unroll
-      for (int i = 0; i < CH; i += 2) {
-        __half2 h;
-        *reinterpret_cast<uint32_t*>(&h) = pk[i >> 1];
-        const float2 f = __half22float2(h);
-        v[i] = valid ? f.x : 0.f;
-        v[i + 1] = valid ? f.y : 0.f;
-      }
-    }
-  } else {
+    // round once (one packed conversion per two values); the column sums describe exactly the values that are stored
     uint32_t pk[CH / 2];
 #pragma unroll
     for (int i = 0; i < CH; i += 2) pk[i >> 1] = pack_bf16x2(v[i], v[i + 1]);
@@ -326,38 +282,31 @@ __device__ __forceinline__ void conv_epilogue_chunk(const ConvGemmParams& p, flo
       for (int i = 0; i < CH; i += 8)
         if (cbase + i < p.cout) *reinterpret_cast<uint4*>(o + i) = make_uint4(pk[i >> 1], pk[(i >> 1) + 1], pk[(i >> 1) + 2], pk[(i >> 1) + 3]);
     }
-    if (need_vals) {
+    if ((p.epi_mode == EPI_BF16_GELU_BWD || p.epi_mode == EPI_BF16_RELU_BWD) && p.stat_sum != nullptr) {
 #pragma unroll
       for (int i = 0; i < CH; i += 2) {
         v[i] = valid ? bf16_lo(pk[i >> 1]) : 0.f;
         v[i + 1] = valid ? bf16_hi(pk[i >> 1]) : 0.f;
       }
+      float cs;
+      if constexpr (CH == 32) cs = warp_colsum32(v, lane);
+      else cs = warp_colsum16(v, lane);
+      if (lane < CH) part_sum[lane] = accumulate ? part_sum[lane] + cs : cs;  // each (warp, column) slot has exactly one writer
     }
-  }
-  if (p.epi_mode == EPI_F16_STATS) {
-    float sq[CH];
-#pragma unroll
-    for (int i = 0; i < CH; ++i) sq[i] = v[i] * v[i];
-    float cs, cq;
-    if constexpr (CH == 32) { cs = warp_colsum32(v, lane); cq = warp_colsum32(sq, lane); }
-    else { cs = warp_colsum16(v, lane); cq = warp_colsum16(sq, lane); }
-    if (lane < CH) {  // each (warp, column) slot has exactly one writer
-      part_sum[lane] = accumulate ? part_sum[lane] + cs : cs;
-      part_sq[lane] = accumulate ? part_sq[lane] + cq : cq;
-    }
-  } else if (EXT && (p.epi_mode == EPI_BF16_GELU_BWD || p.epi_mode == EPI_BF16_RELU_BWD) && p.stat_sum != nullptr) {
-    float cs;
-    if constexpr (CH == 32) cs = warp_colsum32(v, lane);
-    else cs = warp_colsum16(v, lane);
-    if (lane < CH) part_sum[lane] = accumulate ? part_sum[lane] + cs : cs;
   }
 }
 
 // ================================================================================================
 // Persistent kernel: each CTA walks a strided list of 128-pixel tiles for ONE column tile.
 //   warps 0-3, 4-7  two consumer warpgroups.  Warpgroup g computes rows [64 g, 64 g + 64) of the tile with wgmma (accumulator in
-//                   registers) and then runs the epilogue of those rows: the accumulator passes through a per-warpgroup fp32 staging tile
-//                   in shared memory, kCols columns per round, so that every epilogue lane owns one pixel row, as conv_epilogue_chunk expects
+//                   registers) and then runs the epilogue of those rows.  The mode selects one of two epilogues, because the output
+//                   format forces it:
+//                   - TMA store (the 16-bit modes EPI_BF16, EPI_F16, EPI_F16_STATS, EPI_BF16_BN_SILU of EXT = false): the mode's arithmetic
+//                     on the accumulator fragment, stmatrix into a swizzled 16-bit tile, one bulk tensor store of the warpgroup's 64 rows
+//                     (ConvTmaEpiCfg, ConvOutMaps); an addend tile arrives by TMA into the same buffer and is read with ldmatrix
+//                   - staging tile (EPI_F32_BIAS, whose [B, A, 85] rows a tensor map cannot address, and the EXT modes): the accumulator
+//                     passes through a per-warpgroup fp32 tile in shared memory, kCols columns per round, so that every epilogue lane owns
+//                     one pixel row, as conv_epilogue_chunk expects
 //   warp 8          TMA producer: the ring runs ahead across tile boundaries, so the loads of tile i+1 overlap the epilogue of tile i
 // Per-channel statistics are accumulated in shared memory over all tiles of the CTA (one fp64 atomic per channel and CTA instead of per
 // tile); barrier setup and descriptor prefetch are paid once.
@@ -377,7 +326,40 @@ struct ConvEpiCfg {
   static constexpr int kStageBytes = 2 * 64 * kPitch * 4;     // both warpgroups
 };
 
+// Output tile of the TMA-store epilogue: a warpgroup's 64 rows x BLOCK_N 16-bit columns as boxes of at most 64 columns (a swizzled box row
+// is at most 128 bytes), each in the swizzle of its row width (32 / 64 / 128 bytes: stmatrix and ldmatrix are then free of bank conflicts).
+// The buffers live in the bytes of the fp32 staging tile, so shared memory and CTAs per SM are the same on both paths: two per warpgroup
+// where they fit (BN 16 / 32), else one.
+template <int BLOCK_N>
+struct ConvTmaEpiCfg {
+  static constexpr int kBoxCols = BLOCK_N < 64 ? BLOCK_N : 64;
+  static constexpr int kBoxes = BLOCK_N / kBoxCols;
+  static constexpr int kRowBytes = 2 * kBoxCols;  // = the swizzle span
+  static constexpr int kBoxBytes = 64 * kRowBytes;
+  static constexpr int kBufBytes = kBoxes * kBoxBytes;
+  static constexpr int kBufs = 2 * 2 * kBufBytes <= ConvEpiCfg<BLOCK_N>::kStageBytes ? 2 : 1;
+  static_assert(2 * kBufs * kBufBytes <= ConvEpiCfg<BLOCK_N>::kStageBytes, "output tiles must fit in the staging tile's bytes");
+};
+
+// Tensor maps of the TMA-store epilogue: the 16-bit output view and the addend as (c, x, y, n) over the pixel grid of the work items, with
+// the view's own extents, so that TMA clipping drops the columns beyond the view's channels and the pixels beyond the valid grid.  A
+// four-phase data gradient has one map per output-parity phase (ph, pw) at index 2 ph + pw; other launches use index 0.
+struct ConvOutMaps {
+  CUtensorMap out[4];
+  CUtensorMap add[4];
+};
+
 __host__ __device__ constexpr int conv_min_ctas(int block_n, int block_k) { return (block_n >= 128 || block_k == 16) ? 1 : 2; }
+
+// The 64-row half of a (tw, th, tn) pixel tile that warpgroup g stores: the outermost dimension longer than one pixel is halved.  Offsets of
+// half 1 in (x, y, n); the TMA box is the tile with that dimension halved (conv_api.cu).
+__host__ __device__ inline void conv_half_offset(int log_tw, int log_th, int& dx, int& dy, int& dn) {
+  const int log_tn = 7 - log_tw - log_th;
+  dx = dy = dn = 0;
+  if (log_tn > 0) dn = 1 << (log_tn - 1);
+  else if (log_th > 0) dy = 1 << (log_th - 1);
+  else dx = 1 << (log_tw - 1);
+}
 
 // EXT: false = YOLOX training / inference epilogues, true = + ConvNeXt / transformer epilogues
 template <int BLOCK_N, int BLOCK_K, bool EXT>
@@ -385,12 +367,15 @@ template <int BLOCK_N, int BLOCK_K, bool EXT>
 // spilling; one CTA per SM (168 registers) for BN 128 and for BLOCK_K 16 (the deep k-block slots); conv_min_ctas
 __global__ void __launch_bounds__(kConvThreadsP, conv_min_ctas(BLOCK_N, BLOCK_K))
 conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                            const __grid_constant__ ConvGemmParams p, int num_stages, int kb_per_slot, int n_tiles, int m_tiles) {
+                            const __grid_constant__ ConvGemmParams p, const __grid_constant__ ConvOutMaps om, int num_stages, int kb_per_slot,
+                            int n_tiles, int m_tiles) {
   using Cfg = ConvGemmCfg<BLOCK_N, BLOCK_K>;
   using Epi = ConvEpiCfg<BLOCK_N>;
+  using TE = ConvTmaEpiCfg<BLOCK_N>;
+  static_assert(Cfg::kStageBytes % (8 * TE::kRowBytes) == 0, "output tiles must start on a swizzle-pattern boundary");
   constexpr int CH = Epi::kChunk;
   extern __shared__ uint8_t smem_dyn[];
-  __shared__ __align__(8) uint64_t s_bar[2 * kMaxStagesP];
+  __shared__ __align__(8) uint64_t s_bar[2 * kMaxStagesP + 4];  // ring full / empty, then the addend tiles [warpgroup][buffer]
   __shared__ float s_part[4][2][BLOCK_N];
   __shared__ __align__(16) float s_col[2][BLOCK_N];
 
@@ -401,6 +386,8 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
   const int ring_bytes = num_stages * kb_per_slot * Cfg::kStageBytes;
   const uint32_t bar_full = smem_u32(&s_bar[0]);
   const uint32_t bar_empty = smem_u32(&s_bar[kMaxStagesP]);
+  const uint32_t bar_add = smem_u32(&s_bar[2 * kMaxStagesP]);
+  const bool tma_epi = !EXT && p.epi_mode != EPI_F32_BIAS;
 
   const int n_tile = blockIdx.x % n_tiles;
   const int group = blockIdx.x / n_tiles;
@@ -413,6 +400,7 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
       mbar_init(bar_full + 8 * s, 1);
       mbar_init(bar_empty + 8 * s, 2);  // one arrival per consumer warpgroup
     }
+    for (int s = 0; s < 4; ++s) mbar_init(bar_add + 8 * s, 1);
     mbar_fence_init();
   }
   for (int i = threadIdx.x; i < 4 * 2 * BLOCK_N; i += blockDim.x) (&s_part[0][0][0])[i] = 0.f;
@@ -457,7 +445,7 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
     // ===================== consumer warpgroups: MMA, then the epilogue of their 64 rows =====================
     const int g = warp >> 2;         // rows [64 g, 64 g + 64) of the tile
     const int wl = warp & 3;
-    const int q = 2 * g + (wl & 1);  // 32-row quadrant whose epilogue this warp runs
+    const int q = 2 * g + (wl & 1);  // 32-row quadrant whose epilogue (staging path) or statistics (both paths) this warp runs
     const int half = wl >> 1;        // which part of each staged round of columns
     const int mrow = q * 32 + lane;
     const int xl = mrow & ((1 << log_tw) - 1);
@@ -466,6 +454,22 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
     float* const stg = reinterpret_cast<float*>(smem_al + ring_bytes) + g * 64 * Epi::kPitch;
     float* xp = nullptr;
     if (p.xpose) xp = reinterpret_cast<float*>(smem_al + ring_bytes + Epi::kStageBytes) + warp * kXposeWarpFloats;
+    // TMA path: the leader thread of the warpgroup issues, commits and waits for its bulk copies (bulk async-groups are per thread)
+    const bool leader = (threadIdx.x & 127) == 0;
+    const bool add_tile = tma_epi && p.addend != nullptr;
+    const uint32_t obuf = smem_base + ring_bytes + g * TE::kBufs * TE::kBufBytes;
+    // stmatrix / ldmatrix rows of this lane: lanes 8j .. 8j + 7 address matrix j = rows + 8 (j & 1), column block + (j >> 1); the 16-byte
+    // chunk index is XORed with address bits 7 and up (the TMA swizzle of kRowBytes-wide rows)
+    const int srow = 16 * wl + (lane & 7) + 8 * ((lane >> 3) & 1);
+    const uint32_t srow_off = srow * TE::kRowBytes;
+    const uint32_t schunk = (lane >> 4) ^ ((srow_off >> 7) & (TE::kRowBytes / 16 - 1));
+    int hx, hy, hn;
+    conv_half_offset(log_tw, log_th, hx, hy, hn);
+    hx *= g; hy *= g; hn *= g;
+    if (tma_epi && leader) {
+      tma_prefetch_desc(&om.out[0]);
+      if (add_tile) tma_prefetch_desc(&om.add[0]);
+    }
     constexpr uint32_t lcode = gmma_layout_code(Cfg::kSwizzle);
     constexpr uint32_t sbo = 8 * Cfg::kSwizzle;  // 8 rows of one swizzle atom
     float acc[BLOCK_N / 2];
@@ -474,10 +478,28 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
     wgmma_fence_operand(acc);
     int stage = 0;
     uint32_t phase = 0;
-    for (int wi = group; wi < m_tiles; wi += groups) {
+    int it = 0;  // tiles of this CTA so far
+    for (int wi = group; wi < m_tiles; wi += groups, ++it) {
       int m, tap, ntaps, oph, opw;
       conv_decode_work(p, wi, m, tap, ntaps, oph, opw);
       const int num_kb = ntaps * p.cin_blocks;
+      int t = m;
+      const int tw = t % p.tiles_w;
+      t /= p.tiles_w;
+      const int th = t % p.tiles_h;
+      const int tn = t / p.tiles_h;
+      const int w0 = tw << log_tw, h0 = th << log_th, n0 = tn << (7 - log_tw - log_th);
+      const int pm = p.num_phases == 4 ? 2 * oph + opw : 0;
+      const int slot = TE::kBufs == 2 ? (it & 1) : 0;
+      const uint32_t buf = obuf + slot * TE::kBufBytes;
+      const uint32_t abar = bar_add + 8 * (2 * g + slot);
+      if (add_tile && leader) {
+        // the addend tile goes to the buffer that this tile's output will occupy; its latency hides behind the main loop
+        if (TE::kBufs == 1) bulk_wait_read<0>();  // the previous tile's store has read the buffer
+        mbar_expect_tx(abar, TE::kBufBytes);
+#pragma unroll
+        for (int b = 0; b < TE::kBoxes; ++b) tma_load_4d(buf + b * TE::kBoxBytes, &om.add[pm], abar, col0 + 64 * b, w0 + hx, h0 + hy, n0 + hn);
+      }
       int j = 0, prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {  // one wgmma group per k-block; ring slots hold kb_per_slot of them
         if (j == 0) mbar_wait(bar_full + 8 * stage, phase);
@@ -503,46 +525,138 @@ conv_gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __gri
       wgmma_fence_operand(acc);
       mbar_arrive_if(bar_empty + 8 * prev, (threadIdx.x & 127) == 0);
 
-      int t = m;
-      const int tw = t % p.tiles_w;
-      t /= p.tiles_w;
-      const int th = t % p.tiles_h;
-      const int tn = t / p.tiles_h;
-      const int x = (tw << log_tw) + xl, y = (th << log_th) + yl, n = (tn << (7 - log_tw - log_th)) + nl;
-      const bool valid = (x < p.w_valid) && (y < p.h_valid) && (n < p.n_valid);
-      const long long pix_off = (long long)n * p.out_sn + (long long)(y * p.out_mh + oph) * p.out_sh +
-                                (long long)(x * p.out_mw + opw) * p.out_sw;
-      const long long add_off = (long long)n * p.add_sn + (long long)(y * p.out_mh + oph) * p.add_sh +
-                                (long long)(x * p.out_mw + opw) * p.add_sw;
-      float* const r0 = stg + (16 * wl + (lane >> 2)) * Epi::kPitch + 2 * (lane & 3);  // this thread's fragment rows in the staging tile
-      float* const r1 = r0 + 8 * Epi::kPitch;
-      const float* const row_src = stg + ((wl & 1) * 32 + lane) * Epi::kPitch + half * CH;
-#pragma unroll 1
-      for (int r = 0; r < BLOCK_N / Epi::kCols; ++r) {
-        named_bar_sync(1 + g, 128);  // every row of the previous round has been read
+      if (tma_epi) {
+        if (TE::kBufs == 1 && !add_tile) {  // the previous tile's store has read the buffer (with an addend: implied by its arrival)
+          if (leader) bulk_wait_read<0>();
+          named_bar_sync(1 + g, 128);
+        }
+        // fragment: acc[4 i + e] is row 16 wl + lane / 4 + 8 (e >> 1), column 8 i + 2 (lane % 4) + (e & 1) of the warpgroup's rows
+        if (p.epi_mode == EPI_BF16_BN_SILU) {
 #pragma unroll
-        for (int i = 0; i < BLOCK_N / 8; ++i) {
-          if (i / (Epi::kCols / 8) == r) {
-            const int c = (i % (Epi::kCols / 8)) * 8;
-            *reinterpret_cast<float2*>(r0 + c) = make_float2(acc[4 * i], acc[4 * i + 1]);
-            *reinterpret_cast<float2*>(r1 + c) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+          for (int i = 0; i < BLOCK_N / 8; ++i) {
+            const float2 sc = *reinterpret_cast<const float2*>(&s_col[0][8 * i + 2 * (lane & 3)]);
+            const float2 sh = *reinterpret_cast<const float2*>(&s_col[1][8 * i + 2 * (lane & 3)]);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const float u = fmaf(acc[4 * i + e], (e & 1) ? sc.y : sc.x, (e & 1) ? sh.y : sh.x);
+              acc[4 * i + e] = bf16_round(__fdividef(u, 1.f + __expf(-u)));  // rounded before the residual add, as a materialised activation
+            }
           }
         }
-        named_bar_sync(1 + g, 128);
-        const int c = r * Epi::kCols + half * CH;  // tile column of this warp's chunk
-        // chunks at or beyond the last valid output channel are dead (cout not a multiple of the column tile)
-        if (half < Epi::kHalves && col0 + c < p.cout) {
-          float v[CH];
+        if (add_tile) {
+          mbar_wait(abar, (it / TE::kBufs) & 1);
 #pragma unroll
-          for (int i = 0; i < CH; i += 4) {
-            const float4 f = *reinterpret_cast<const float4*>(row_src + i);
-            v[i] = f.x; v[i + 1] = f.y; v[i + 2] = f.z; v[i + 3] = f.w;
+          for (int i = 0; i < BLOCK_N / 8; i += 2) {
+            uint32_t a[4];
+            ldmatrix_x4(buf + (i >> 3) * TE::kBoxBytes + srow_off + (((i & 7) ^ schunk) << 4), a[0], a[1], a[2], a[3]);
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+              acc[4 * i + 2 * r] += bf16_lo(a[r]);
+              acc[4 * i + 2 * r + 1] += bf16_hi(a[r]);
+            }
           }
-          conv_epilogue_chunk<CH, EXT>(p, v, valid, pix_off, add_off, col0 + c, lane, &s_part[q][0][c], &s_part[q][1][c], true, &s_col[0][c],
-                                       &s_col[1][c], xp);
+        }
+        // round once: pk[2 i] holds row lane / 4 and pk[2 i + 1] row lane / 4 + 8 of column pair 8 i + 2 (lane % 4)
+        uint32_t pk[BLOCK_N / 4];
+        if (p.epi_mode == EPI_F16 || p.epi_mode == EPI_F16_STATS) {
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 4; ++i) pk[i] = pack_f16x2(acc[2 * i], acc[2 * i + 1]);
+        } else {
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 4; ++i) pk[i] = pack_bf16x2(acc[2 * i], acc[2 * i + 1]);
+        }
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 8; i += 2)
+          stmatrix_x4(buf + (i >> 3) * TE::kBoxBytes + srow_off + (((i & 7) ^ schunk) << 4), pk[2 * i], pk[2 * i + 1], pk[2 * i + 2], pk[2 * i + 3]);
+        fence_proxy_async_smem();
+        // two buffers: the previous tile's store has read the other one before any thread passes this barrier, so the next tile may fill it
+        if (TE::kBufs == 2 && leader) bulk_wait_read<0>();
+        named_bar_sync(1 + g, 128);
+        if (leader) {
+#pragma unroll
+          for (int b = 0; b < TE::kBoxes; ++b) tma_store_4d(&om.out[pm], buf + b * TE::kBoxBytes, col0 + 64 * b, w0 + hx, h0 + hy, n0 + hn);
+          bulk_commit();
+        }
+        if (p.epi_mode == EPI_F16_STATS) {
+          // Σ and Σ² of the stored values, read back from the output tile (the store only reads it as well; the next write to this buffer
+          // follows a barrier that every thread passes after these reads), in exactly the order of the staging path: one pixel row per lane
+          // and 16 or 32 columns per warp, a butterfly over the 32 rows of a quadrant, per-quadrant sums over the CTA's tiles.  The sums are
+          // then the same fp32 additions as on the parent's path, and a training step computes the same BatchNorm statistics bit for bit.
+          const bool valid = w0 + xl < p.w_valid && h0 + yl < p.h_valid && n0 + nl < p.n_valid;
+          const uint32_t row = (wl & 1) * 32 + lane;  // this lane's row of the warpgroup's tile
+          const uint32_t rxor = ((row * TE::kRowBytes) >> 7) & (TE::kRowBytes / 16 - 1);
+#pragma unroll 1
+          for (int r = 0; r < BLOCK_N / Epi::kCols; ++r) {
+            const int c = r * Epi::kCols + half * CH;
+            if (half < Epi::kHalves && col0 + c < p.cout) {
+              float v[CH], sq[CH];
+#pragma unroll
+              for (int i = 0; i < CH; i += 8) {
+                const int cc = c + i;
+                uint4 u;
+                asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+                             : "=r"(u.x), "=r"(u.y), "=r"(u.z), "=r"(u.w)
+                             : "r"(buf + (cc / TE::kBoxCols) * TE::kBoxBytes + row * TE::kRowBytes + ((((cc % TE::kBoxCols) >> 3) ^ rxor) << 4))
+                             : "memory");
+                const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                  __half2 hv;
+                  *reinterpret_cast<uint32_t*>(&hv) = w4[j];
+                  const float2 fv = __half22float2(hv);
+                  v[i + 2 * j] = valid ? fv.x : 0.f;
+                  v[i + 2 * j + 1] = valid ? fv.y : 0.f;
+                }
+              }
+#pragma unroll
+              for (int i = 0; i < CH; ++i) sq[i] = v[i] * v[i];
+              float cs, cq;
+              if constexpr (CH == 32) { cs = warp_colsum32(v, lane); cq = warp_colsum32(sq, lane); }
+              else { cs = warp_colsum16(v, lane); cq = warp_colsum16(sq, lane); }
+              if (lane < CH) {  // each (quadrant, column) slot has exactly one writer
+                s_part[q][0][c + lane] += cs;
+                s_part[q][1][c + lane] += cq;
+              }
+            }
+          }
+        }
+      } else {
+        const int x = w0 + xl, y = h0 + yl, n = n0 + nl;
+        const bool valid = (x < p.w_valid) && (y < p.h_valid) && (n < p.n_valid);
+        const long long pix_off = (long long)n * p.out_sn + (long long)(y * p.out_mh + oph) * p.out_sh +
+                                  (long long)(x * p.out_mw + opw) * p.out_sw;
+        const long long add_off = (long long)n * p.add_sn + (long long)(y * p.out_mh + oph) * p.add_sh +
+                                  (long long)(x * p.out_mw + opw) * p.add_sw;
+        float* const r0 = stg + (16 * wl + (lane >> 2)) * Epi::kPitch + 2 * (lane & 3);  // this thread's fragment rows in the staging tile
+        float* const r1 = r0 + 8 * Epi::kPitch;
+        const float* const row_src = stg + ((wl & 1) * 32 + lane) * Epi::kPitch + half * CH;
+#pragma unroll 1
+        for (int r = 0; r < BLOCK_N / Epi::kCols; ++r) {
+          named_bar_sync(1 + g, 128);  // every row of the previous round has been read
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 8; ++i) {
+            if (i / (Epi::kCols / 8) == r) {
+              const int c = (i % (Epi::kCols / 8)) * 8;
+              *reinterpret_cast<float2*>(r0 + c) = make_float2(acc[4 * i], acc[4 * i + 1]);
+              *reinterpret_cast<float2*>(r1 + c) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+            }
+          }
+          named_bar_sync(1 + g, 128);
+          const int c = r * Epi::kCols + half * CH;  // tile column of this warp's chunk
+          // chunks at or beyond the last valid output channel are dead (cout not a multiple of the column tile)
+          if (half < Epi::kHalves && col0 + c < p.cout) {
+            float v[CH];
+#pragma unroll
+            for (int i = 0; i < CH; i += 4) {
+              const float4 f = *reinterpret_cast<const float4*>(row_src + i);
+              v[i] = f.x; v[i + 1] = f.y; v[i + 2] = f.z; v[i + 3] = f.w;
+            }
+            conv_epilogue_chunk<CH, EXT>(p, v, valid, pix_off, add_off, col0 + c, lane, &s_part[q][0][c], true, &s_col[0][c], &s_col[1][c], xp);
+          }
         }
       }
     }
+    if (tma_epi && leader) bulk_wait_all();  // the stores have completed before the CTA's shared memory is released
   }
 
   __syncthreads();

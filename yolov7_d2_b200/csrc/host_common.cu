@@ -107,6 +107,23 @@ int make_mat_map(CUtensorMap* m, const void* ptr, long long rows, long long cols
   return 0;
 }
 
+int make_pix_map(CUtensorMap* m, const void* base, int c, int w, int h, int n, long long sx, long long sy, long long sn, int box_c, int bw, int bh,
+                 int bn) {
+  EncodeTiledFn fn = encode_fn();
+  YB_REQUIRE(fn != nullptr, YB200_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  YB_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && sx % 8 == 0 && sy % 8 == 0 && sn % 8 == 0, YB200_ERR_INVALID,
+             "16-bit pixel view must start 16B aligned with strides that are multiples of 8 elements (strides %lld, %lld, %lld)", sx, sy, sn);
+  cuuint64_t gdim[4] = {static_cast<cuuint64_t>(c), static_cast<cuuint64_t>(w), static_cast<cuuint64_t>(h), static_cast<cuuint64_t>(n)};
+  cuuint64_t gstr[3] = {static_cast<cuuint64_t>(sx) * 2, static_cast<cuuint64_t>(sy) * 2, static_cast<cuuint64_t>(sn) * 2};
+  cuuint32_t box[4] = {static_cast<cuuint32_t>(box_c), static_cast<cuuint32_t>(bw), static_cast<cuuint32_t>(bh), static_cast<cuuint32_t>(bn)};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT16, 4, const_cast<void*>(base), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  swizzle_for(box_c * 2), CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  YB_REQUIRE(r == CUDA_SUCCESS, YB200_ERR_CUDA, "cuTensorMapEncodeTiled(pixels c=%d w=%d h=%d n=%d box=%d,%d,%d,%d) failed: %d", c, w, h, n,
+             box_c, bw, bh, bn, static_cast<int>(r));
+  return 0;
+}
+
 void choose_tile(int n, int h, int w, int npix, int* log_tw, int* log_th) {
   const int lp = ilog2(npix);
   long long best = -1;

@@ -67,6 +67,11 @@ inline bool same_geometry(const yb200_act* a, const yb200_act* b) { return same_
 int make_act_map(CUtensorMap* m, const yb200_act& a, bool space_to_depth, int box_c, int tw, int th, int tn);
 // 2-D K-major bf16 matrix [rows][cols], box [box_rows][box_cols]
 int make_mat_map(CUtensorMap* m, const void* ptr, long long rows, long long cols, int box_rows, int box_cols);
+// 4-D (c, x, y, n) view of 16-bit values: element (c, x, y, n) at base + c + x * sx + y * sy + n * sn (strides in elements), extents
+// (c, w, h, n); box (box_c, bw, bh, bn) in the swizzle of its 2 * box_c-byte rows.  Rejects a base that is not 16-byte aligned and strides
+// that are not multiples of 8 elements (TMA requirements).
+int make_pix_map(CUtensorMap* m, const void* base, int c, int w, int h, int n, long long sx, long long sy, long long sn, int box_c, int bw, int bh,
+                 int bn);
 
 // pick (tw, th, tn) with tw*th*tn == npix (power of two) minimising padded pixels for an (n,h,w) grid
 void choose_tile(int n, int h, int w, int npix, int* log_tw, int* log_th);
